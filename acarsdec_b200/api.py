@@ -99,6 +99,10 @@ ABI = [
     ("acb_fast_plan_cs16", C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p]),
     ("acb_fast_plan_air", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p]),
     ("acb_build_h", None, [C.c_void_p]),
+    ("acb_build_lowpass", C.c_int, [C.c_int, C.c_int, C.c_void_p]),
+    ("acb_build_wf_lp", None, [C.c_int, C.c_uint, C.c_int, C.c_int, C.c_void_p]),
+    ("acb_cs16_build_wf_lp", None, [C.c_int, C.c_uint, C.c_uint, C.c_int, C.c_int, C.c_void_p]),
+    ("acb_air_build_wf_lp", None, [C.c_int, C.c_int, C.c_uint, C.c_int, C.c_void_p]),
     ("acb_create", C.c_int, [C.POINTER(Config), C.POINTER(C.c_void_p)]),
     ("acb_destroy", None, [C.c_void_p]),
     ("acb_last_error", C.c_char_p, []),
@@ -314,6 +318,44 @@ def build_h() -> np.ndarray:
     h = np.empty(133, dtype=np.float32)
     load().acb_build_h(h.ctypes.data)
     return h
+
+
+MAXTAPS_PER_K = 16
+
+
+def build_lowpass(K: int, taps: int) -> np.ndarray:
+    """The channel-filter prototype of an overlapping-window context (taps > K): Kaiser-windowed (beta 6) ideal
+    low-pass at 6.25 kHz, sum 1, float32 (acb_build_lowpass)."""
+    h = np.empty(taps, dtype=np.float32)
+    _check(load(), load().acb_build_lowpass(K, taps, h.ctypes.data))
+    return h
+
+
+def build_wf_lp(K: int, taps: int, freqs_mhz) -> np.ndarray:
+    """(nch, 2*taps) tables acb_set_plan builds for a u8 context with taps > K (acb_build_wf_lp)."""
+    lib = load()
+    _, fr, fc = plan(K, freqs_mhz)
+    out = np.empty((len(fr), 2 * taps), dtype=np.float32)
+    for i, f in enumerate(fr):
+        lib.acb_build_wf_lp(f, fc, K, taps, out[i].ctypes.data)
+    return out
+
+
+def build_wf_cs16_lp(variant: int, K: int, taps: int, freqs_hz, fc_hz: int) -> np.ndarray:
+    lib = load()
+    out = np.empty((len(freqs_hz), 2 * taps), dtype=np.float32)
+    for i, f in enumerate(freqs_hz):
+        lib.acb_cs16_build_wf_lp(variant, int(f), int(fc_hz), K, taps, out[i].ctypes.data)
+    return out
+
+
+def build_wf_air_lp(rate: int, taps: int, freqs_mhz) -> np.ndarray:
+    lib = load()
+    fd, fc, _ = air_plan(rate, freqs_mhz)
+    out = np.empty((len(fd), 2 * taps), dtype=np.float32)
+    for i, f in enumerate(fd):
+        lib.acb_air_build_wf_lp(f, fc, rate, taps, out[i].ctypes.data)
+    return out
 
 
 def block_fec(msg: Msg):

@@ -61,10 +61,22 @@ constexpr int CH_GROUP = 8;           /* channels accumulated per pass */
 struct CUstream_st;
 namespace acb {
 enum InputKind { IN_KIND_U8IQ = 0, IN_KIND_F32REAL = 1, IN_KIND_CS16IQ = 2 };
+/* Input history of a context with taps > K (the overlapping window): stream s's last `hpad` samples before the submit
+ * start at (const char *)base + s*stride.  hpad = 0: taps <= K, no history.  pos0 = the submit's first output row,
+ * counted from acb_create / acb_reset (rows whose window reaches before the stream start omit those terms). */
+struct Hist {
+	const void *base;
+	size_t stride;
+	int hpad;
+	unsigned long long pos0;
+};
 int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
-                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, CUstream_st *stream);
+                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, CUstream_st *stream);
 int launch_channelize_generic(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
                               int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp, CUstream_st *stream);
+int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
+                                  int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
+                                  const Hist &h, CUstream_st *stream);
 int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
                  RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, CUstream_st *stream);
 int demod_pick_lanes(long long nchains, int sm_count);

@@ -319,6 +319,25 @@ void demodMSK(channel_t *ch, int len)
 	pthread_mutex_unlock(&one_mtx);
 }
 
+/* ACARSDEC_B200_TAPS=<n>: the channel filter length of every front-end (acb_config_t.taps).  Unset, or n == K: the
+ * reference's boxcar; K < n <= ACB_MAXTAPS_PER_K*K: the planner's low-pass over an overlapping window
+ * (acb_build_lowpass), which keeps a strong neighbour channel out of a weak one.  Anything else is an init error. */
+static int env_taps(int K, int *taps)
+{
+	const char *e = getenv("ACARSDEC_B200_TAPS");
+	*taps = 0;
+	if (!e || !*e) return 0;
+	char *end;
+	const long v = strtol(e, &end, 10);
+	if (*end || v < K || v > (long)ACB_MAXTAPS_PER_K * K) {
+		fprintf(stderr, "acarsdec_b200: ACARSDEC_B200_TAPS=%s: need a number of taps from %d (the reference's boxcar) to %d\n",
+		        e, K, ACB_MAXTAPS_PER_K * K);
+		return -1;
+	}
+	*taps = v == K ? 0 : (int)v;
+	return 0;
+}
+
 /* ---------------------------------------------------------------- RTL front-end on a capture file */
 
 #ifdef WITH_RTL
@@ -400,6 +419,7 @@ int initRtl(char **argv, int optind)
 	const char *e = getenv("ACARSDEC_B200_BLOCKS");
 	if (e && atoi(e) > 0) rtl_batch = atoi(e);
 	acb_config_t cfg = { 0, rtlMult, 1, (int)nbch, rtl_batch, 0, 0 };
+	if (env_taps(rtlMult, &cfg.taps)) return 1;
 	int devs[MAXNBCHANNELS];
 	const int ndev = parse_devices(devs, MAXNBCHANNELS);
 	if (acb_multi_create(&cfg, devs, ndev, ACB_MULTI_SPLIT_CHANNELS, &rtl_ctx) != ACB_OK) {
@@ -422,7 +442,8 @@ int initRtl(char **argv, int optind)
 		for (int i = 0; i < rtlMult; i++)
 			ch->wf[i] = wf[((size_t)n * rtlMult + i) * 2] + wf[((size_t)n * rtlMult + i) * 2 + 1] * I;
 	}
-	int rc = acb_multi_set_wf(rtl_ctx, 0, wf, (int)nbch);
+	/* channel[].wf keeps the reference's K-entry table either way; with a longer filter the library plans its own */
+	int rc = cfg.taps ? acb_multi_set_plan(rtl_ctx, 0, Fd, (int)nbch, NULL) : acb_multi_set_wf(rtl_ctx, 0, wf, (int)nbch);
 	free(wf);
 	if (rc != ACB_OK) {
 		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
@@ -545,6 +566,7 @@ int initAirspy(char **argv, int optind)
 	if (verbose) fprintf(stderr, "Using %d sampling rate\nSet freq. to %d hz\n", air_rate, Fc);
 	const int maxblk = (AIR_TRANSFER * 8 / (int)air_mult) / RTLOUTBUFSZ + 2;
 	acb_config_t cfg = { 0, (int)air_mult, 1, (int)nbch, maxblk, ACB_FLAG_REAL_INPUT, 0 };
+	if (env_taps((int)air_mult, &cfg.taps)) return -1;
 	if ((e = getenv("ACARSDEC_B200_DEVICE"))) cfg.device = atoi(e);
 	if (acb_create(&cfg, &air_ctx) != ACB_OK) {
 		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
@@ -564,7 +586,7 @@ int initAirspy(char **argv, int optind)
 		for (unsigned i = 0; i < air_mult; i++)
 			ch->wf[i] = wf[((size_t)n * air_mult + i) * 2] + wf[((size_t)n * air_mult + i) * 2 + 1] * I;
 	}
-	int rc = acb_set_wf(air_ctx, 0, wf, (int)nbch);
+	int rc = cfg.taps ? acb_set_plan_air(air_ctx, 0, Fd, (int)nbch, NULL) : acb_set_wf(air_ctx, 0, wf, (int)nbch);
 	free(wf);
 	if (rc != ACB_OK) { fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error()); return -1; }
 	return 0;
@@ -648,6 +670,7 @@ static int cs16_setup(const char *path, char **argv, int optind, int mult, int v
 	}
 	if (nbch == 0) { fprintf(stderr, "Need a least one frequency\n"); return 1; }
 	acb_config_t cfg = { 0, mult, 1, (int)nbch, CS_BATCH, ACB_FLAG_CS16_INPUT, 0 };
+	if (env_taps(mult, &cfg.taps)) return -1;
 	const char *e = getenv("ACARSDEC_B200_DEVICE");
 	if (e) cfg.device = atoi(e);
 	if (acb_create(&cfg, &cs_ctx) != ACB_OK) {

@@ -133,11 +133,14 @@ struct acb_ctx {
 	bool overflowed;
 	acb_stats_t stats;
 	bool use_generic;
-	int taps;                    /* FIR length actually applied per output row (<= K) */
-	int taps_pad;                /* taps rounded up to whole 16-byte units of input (zero weights) */
+	int taps;                    /* FIR length per output row (<= ACB_MAXTAPS_PER_K * K) */
+	int taps_pad;                /* taps <= K: taps rounded up to whole 16-byte units of input (zero weights behind);
+	                                taps > K: K + hpad (zero weights in front) */
+	int hpad;                    /* taps > K: H = taps - K rounded up to whole 16-byte units of input; else 0 */
+	uint8_t *d_hist;             /* u8 IQ, taps > K: per stream, the last hpad samples of its input so far */
 	int in_kind;                 /* IN_KIND_*: u8 IQ blocks | float32 real (air.c) | CS16 IQ (soapy.c, sdrplay.c) */
 	bool real_input;             /* in_kind != u8: 4-byte input elements, arbitrary submit lengths, carried remainder */
-	float *d_real[2];            /* per stream: [carry + new samples], alternating per submit */
+	float *d_real[2];            /* per stream: [hpad history + carry + new samples], alternating per submit */
 	size_t real_cap;             /* floats per stream in d_real */
 	size_t carry;                /* samples of every stream not yet consumed (< K) */
 	int real_buf;
@@ -219,6 +222,14 @@ static int reset_states(acb_ctx *c)
 	 * so nothing on the legacy stream (plain cudaMemset/cudaMemcpy) is ordered against them */
 	if (int r = upload(c, c->d_state, init.data(), n * sizeof(ChainState))) return r;
 	for (int i = 0; i < NPIPE; i++) CU(cudaMemsetAsync(c->d_ctl[i], 0, sizeof(RingCtl), c->s_copy));
+	/* taps > K: the history restarts.  int16 and float32 zero convert to 0, so zero history is the definition's
+	 * omitted terms exactly (the same +-0 argument as for the front padding, acb_create).  A zero u8 byte converts to
+	 * -127.37: the first rows after a reset are recomputed with the omitted terms (run_kernels), the zeros here only
+	 * keep the pipeline kernel's discarded values finite. */
+	if (c->d_hist) CU(cudaMemsetAsync(c->d_hist, 0, (size_t)c->cfg.nstreams * c->hpad * 2, c->s_copy));
+	if (c->hpad && c->real_input)
+		for (int i = 0; i < 2; i++)
+			CU(cudaMemset2DAsync(c->d_real[i], c->real_cap * sizeof(float), 0, (size_t)c->hpad * sizeof(float), c->cfg.nstreams, c->s_copy));
 	CU(cudaStreamSynchronize(c->s_copy));
 	c->pos = 0;
 	c->carry = 0;
@@ -236,7 +247,8 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	if (!cfg || !out) return fail(ACB_ERR_ARG, "null argument");
 	if (cfg->K < 1 || cfg->K > ACB_MAXK) return fail(ACB_ERR_ARG, "K=%d out of range 1..%d", cfg->K, ACB_MAXK);
 	if (cfg->nstreams < 1 || cfg->nch < 1 || cfg->max_blocks < 1) return fail(ACB_ERR_ARG, "nstreams/nch/max_blocks must be >= 1");
-	if (cfg->taps < 0 || cfg->taps > cfg->K) return fail(ACB_ERR_ARG, "taps=%d must be 0 (= K) or 1..K=%d", cfg->taps, cfg->K);
+	if (cfg->taps < 0 || cfg->taps > ACB_MAXTAPS_PER_K * cfg->K)
+		return fail(ACB_ERR_ARG, "taps=%d must be 0 (= K) or 1..%d*K=%d", cfg->taps, ACB_MAXTAPS_PER_K, ACB_MAXTAPS_PER_K * cfg->K);
 	if ((cfg->flags & ACB_FLAG_REAL_INPUT) && (cfg->flags & ACB_FLAG_CS16_INPUT)) return fail(ACB_ERR_ARG, "REAL_INPUT and CS16_INPUT are exclusive");
 	int ndev = 0;
 	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
@@ -258,9 +270,22 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->taps = cfg->taps ? cfg->taps : cfg->K;
 	{
 		const int per_unit = c->real_input ? 4 : 8;          /* taps per 16 bytes of input (4-byte vs 2-byte taps) */
-		c->taps_pad = c->use_generic ? c->taps : (c->taps + per_unit - 1) / per_unit * per_unit;
-		if (c->taps_pad > cfg->K) c->taps_pad = cfg->K;      /* K itself is a multiple of per_unit here */
+		c->hpad = 0;
+		if (c->taps > cfg->K) {
+			/* overlapping window: H = taps - K samples of the previous rows, rounded up to whole units and padded in
+			 * FRONT with zero weights (acb_set_wf).  Leading zero-weight terms leave the sum unchanged: the accumulator
+			 * starts at +0, each such term is a product with a zero weight, i.e. +-0 (finite input), and +0 + (+-0) = +0
+			 * in round-to-nearest, so the accumulator is still exactly +0 when the first real term p arrives, and
+			 * +0 + p = p is what the unpadded sum starts with.  That holds for any K, so the generic kernel uses the same
+			 * layout. */
+			c->hpad = (c->taps - cfg->K + per_unit - 1) / per_unit * per_unit;
+			c->taps_pad = cfg->K + c->hpad;
+		} else {
+			c->taps_pad = c->use_generic ? c->taps : (c->taps + per_unit - 1) / per_unit * per_unit;
+			if (c->taps_pad > cfg->K) c->taps_pad = cfg->K;      /* K itself is a multiple of per_unit here */
+		}
 	}
+	c->d_hist = nullptr;
 	c->d_real[0] = c->d_real[1] = nullptr;
 	c->d_planar = nullptr;
 	c->planar_cap = 0;
@@ -297,8 +322,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		c->buf_used[i] = false;
 		if (!(cfg->flags & ACB_FLAG_NO_INPUT_STAGING) && !c->real_input) CU(cudaMalloc(&c->d_iq[i], in_bytes));
 		if (c->real_input) {
-			/* room for the carried remainder (< K) plus one submit, rounded so streams stay 32-B aligned */
-			c->real_cap = (((size_t)cfg->max_blocks * OUTBLK + 1) * cfg->K + 7) & ~(size_t)7;     /* streams 32-B aligned: whole sectors per chunk */
+			/* room for the history (taps > K), the carried remainder (< K) plus one submit, rounded so streams stay
+			 * 32-B aligned */
+			c->real_cap = (((size_t)cfg->max_blocks * OUTBLK + 1) * cfg->K + c->hpad + 7) & ~(size_t)7;     /* streams 32-B aligned: whole sectors per chunk */
 			/* + 32 rows: the fast CS16 / real-input kernels fetch whole tiles of up to 32 rows, the last one may reach past the last row */
 			CU(cudaMalloc(&c->d_real[i], ((size_t)cfg->nstreams * c->real_cap + 32 * (size_t)cfg->K) * sizeof(float)));
 			CU(cudaEventCreateWithFlags(&c->ev_real_free[i], cudaEventDisableTiming));
@@ -308,6 +334,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaEventCreateWithFlags(&c->ev_consumed[i], cudaEventDisableTiming));
 	}
 	if (c->real_input) CU(cudaEventCreateWithFlags(&c->ev_real_copied, cudaEventDisableTiming));
+	/* u8 IQ history: its own buffer (acb_submit_device copies no input).  The streaming kinds keep theirs in front of
+	 * the carried remainder in d_real. */
+	if (c->hpad && !c->real_input) CU(cudaMalloc(&c->d_hist, (size_t)cfg->nstreams * c->hpad * 2));
 	const size_t wf_floats = (size_t)cfg->nstreams * c->ngrp * c->taps_pad * CH_GROUP * (c->in_kind == IN_KIND_F32REAL ? 2 : 4);
 	CU(cudaMalloc(&c->d_wf4, wf_floats * sizeof(float)));
 	CU(cudaMemsetAsync(c->d_wf4, 0, wf_floats * sizeof(float), c->s_copy));
@@ -398,6 +427,7 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 		for (auto &e : c->ev_free) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); cudaEventDestroy(e.b2); cudaEventDestroy(e.c); }
 		if (c->ev_real_copied) cudaEventDestroy(c->ev_real_copied);
 		cudaFree(c->d_planar);
+		cudaFree(c->d_hist);
 		cudaFree(c->d_wf4); cudaFree(c->d_state);
 		cudaFree(c->d_tw); cudaFree(c->d_twmeta);
 		for (int i = 0; i < NPIPE; i++) {
@@ -431,13 +461,14 @@ extern "C" int acb_set_wf(acb_ctx_t *c, int stream, const float *wf, int nch)
 	if (stream < 0 || stream >= c->cfg.nstreams || nch != c->cfg.nch) return fail(ACB_ERR_ARG, "stream/nch mismatch");
 	if (int r = ctx_use(c)) return r;
 	const int T = c->taps, TP = c->taps_pad;      /* taps beyond T keep zero weights: D + (+0) = D */
+	const int lead = c->hpad ? TP - T : 0;        /* taps > K: the padding goes in front (acb_create) */
 	const int W = c->in_kind == IN_KIND_F32REAL ? 2 : 4;
 	std::vector<float> t((size_t)c->ngrp * TP * CH_GROUP * W, 0.0f);
 	for (int ch = 0; ch < nch; ch++) {
 		const int g = ch / CH_GROUP, cc = ch % CH_GROUP;
 		for (int ind = 0; ind < T; ind++) {
 			const float re = wf[((size_t)ch * T + ind) * 2], im = wf[((size_t)ch * T + ind) * 2 + 1];
-			float *o = &t[(((size_t)g * TP + ind) * CH_GROUP + cc) * W];
+			float *o = &t[(((size_t)g * TP + lead + ind) * CH_GROUP + cc) * W];
 			o[0] = re; o[1] = im;
 			if (W == 4) { o[2] = -im; o[3] = re; }            /* (c, d, -d, c): see cmac() */
 		}
@@ -482,11 +513,14 @@ extern "C" int acb_set_plan_at(acb_ctx_t *c, int stream, const unsigned *freqs_h
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
 	if (nch != c->cfg.nch) return fail(ACB_ERR_ARG, "nch mismatch");
 	if (c->real_input) return fail(ACB_ERR_ARG, "not a u8-IQ context: use acb_set_plan_air / acb_set_plan_cs16");
-	if (c->taps != c->cfg.K) return fail(ACB_ERR_ARG, "taps != K: the reference planner builds K-tap tables; supply yours with acb_set_wf");
+	if (c->taps < c->cfg.K) return fail(ACB_ERR_ARG, "taps < K: the planners build K-tap or low-pass tables only; supply yours with acb_set_wf");
 	if (fc == 0) return fail(ACB_ERR_PLAN, "centre frequency 0");
-	std::vector<float> wf((size_t)nch * c->cfg.K * 2);
-	for (int ch = 0; ch < nch; ch++)
-		acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, &wf[(size_t)ch * c->cfg.K * 2]);
+	const int T = c->taps;                      /* K, or the low-pass length of an overlapping-window context */
+	std::vector<float> wf((size_t)nch * T * 2);
+	for (int ch = 0; ch < nch; ch++) {
+		if (c->hpad) acb_build_wf_lp(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, T, &wf[(size_t)ch * T * 2]);
+		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
+	}
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
 	if (!c->fast) return ACB_OK;
 	/* Fast form: per-channel bin numbers and twiddles, when every channel sits on the raster */
@@ -731,6 +765,16 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		bool dft = c->fast;                         /* every stream planned on the raster? */
 		for (int s = 0; dft && s < c->cfg.nstreams; s++) dft = c->fast_ok[s] != 0;
 		bool all_rows = false;                       /* the fast CS16 kernel takes partial blocks too */
+		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
+		 * for the streaming kinds (submit4) */
+		Hist hist{ nullptr, 0, c->hpad, c->pos };
+		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
+			hist.base = c->d_hist;
+			hist.stride = (size_t)c->hpad * 2;
+		} else if (c->hpad) {
+			hist.base = d_iq - (size_t)c->hpad * 4;
+			hist.stride = stride;
+		}
 		if (dft && c->in_kind == IN_KIND_F32REAL && !c->use_generic) {
 			r = launch_channelize_rdft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
 			c->stats.kernel_launches++;
@@ -746,13 +790,38 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			c->stats.kernel_launches++;
 			c->stats.fast_chan_launches++;
 		} else if (fast) {
-			r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp, c->s_comp);
+			r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp,
+			                      hist, c->s_comp);
 			c->stats.kernel_launches++;
 		}
 		if (!r && !all_rows && nsamp > fast * OUTBLK) {
-			r = launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
-			                              (size_t)fast * OUTBLK, (size_t)nsamp - (size_t)fast * OUTBLK, (size_t)nsamp, c->s_comp);
+			const size_t row0 = (size_t)fast * OUTBLK, nrows = (size_t)nsamp - row0;
+			r = c->hpad ? launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch,
+			                                            c->cfg.nstreams, row0, nrows, (size_t)nsamp, hist, c->s_comp)
+			            : launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
+			                                        row0, nrows, (size_t)nsamp, c->s_comp);
 			c->stats.kernel_launches++;
+		}
+		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
+			/* u8 history: the pipeline kernel read zero bytes (-127.37 after conversion) for the samples before the stream
+			 * start; the rows whose window reaches there — at most ceil(H/K) <= 16 rows of the first submit after
+			 * create / reset — are recomputed with those terms omitted */
+			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
+			const unsigned long long lead = (H + K - 1) / K;
+			if (!r && fast && c->pos < lead) {
+				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
+				                                  0, (size_t)std::min<unsigned long long>(lead - c->pos, (unsigned long long)nsamp), (size_t)nsamp,
+				                                  hist, c->s_comp);
+				c->stats.kernel_launches++;
+			}
+			/* the input's last hpad samples are the next submit's history; the copy follows K1 on the same stream, so
+			 * K1 of the next submit sees it and the input-lifetime event below covers it */
+			const size_t hb = (size_t)c->hpad * 2, len = (size_t)nblk * c->blk_bytes;
+			if (!r) {
+				r = c->cfg.nstreams == 1 ? (int)cudaMemcpyAsync(c->d_hist, d_iq + len - hb, hb, cudaMemcpyDeviceToDevice, c->s_comp)
+				                         : (int)cudaMemcpy2DAsync(c->d_hist, hb, d_iq + len - hb, stride, hb, c->cfg.nstreams,
+				                                                  cudaMemcpyDeviceToDevice, c->s_comp);
+			}
 		}
 		if (r) return fail(ACB_ERR_CUDA, "channelizer launch: %s", cudaGetErrorString((cudaError_t)r));
 		c->stats.chan_launches++;
@@ -884,15 +953,16 @@ static std::vector<unsigned long long> stream_groups(const acb_ctx *c, size_t no
 static int submit4(acb_ctx *c, const void *x, const void *x2, size_t stride_samples, size_t nsamples)
 {
 	if (int r = ctx_use(c)) return r;
-	const size_t K = (size_t)c->cfg.K, total = c->carry + nsamples;
+	const size_t K = (size_t)c->cfg.K, total = c->carry + nsamples, hp = (size_t)c->hpad;
 	const size_t nout = total / K;
-	if (nsamples == 0 || total > c->real_cap || nout > (size_t)c->cfg.max_blocks * OUTBLK)
+	if (nsamples == 0 || hp + total > c->real_cap || nout > (size_t)c->cfg.max_blocks * OUTBLK)
 		return fail(ACB_ERR_ARG, "nsamples=%zu exceeds max_blocks*1024*K", nsamples);
 	if (c->cfg.nstreams > 1 && stride_samples < nsamples) return fail(ACB_ERR_ARG, "stream stride smaller than one stream's input");
 	const int b = c->real_buf;
 	/* The copy runs on the copy stream, so the H2D of submit i+1 overlaps the channelizer of submit i.
-	 * d_real[b] was last read by the channelizer two submits ago and by the copy that moved its tail on. */
-	float *buf = c->d_real[b];
+	 * d_real[b] was last read by the channelizer two submits ago and by the copy that moved its tail on.
+	 * taps > K: the first hp samples of each stream are its history, rows start behind them. */
+	float *const buf0 = c->d_real[b], *const buf = buf0 + hp;
 	if (c->real_used[b]) CU(cudaStreamWaitEvent(c->s_copy, c->ev_real_free[b], 0));
 	if (!x2) {
 		CU(cudaMemcpy2DAsync(buf + c->carry, c->real_cap * sizeof(float), x, stride_samples * sizeof(float),
@@ -922,11 +992,12 @@ static int submit4(acb_ctx *c, const void *x, const void *x2, size_t stride_samp
 			return r;
 		c->pos += nout;
 		/* the unconsumed tail (air.c:329-334 / soapy.c:238-252 keep a partial sum instead: same
-		 * arithmetic order) moves to the front of the other buffer */
-		if (rem) {
+		 * arithmetic order) moves to the front of the other buffer, behind the hp samples before it (the next
+		 * submit's history, taps > K) */
+		if (rem + hp) {
 			if (c->real_used[b ^ 1]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_real_free[b ^ 1], 0));
-			CU(cudaMemcpy2DAsync(c->d_real[b ^ 1], c->real_cap * sizeof(float), buf + nout * K, c->real_cap * sizeof(float),
-			                     rem * sizeof(float), c->cfg.nstreams, cudaMemcpyDeviceToDevice, c->s_comp));
+			CU(cudaMemcpy2DAsync(c->d_real[b ^ 1], c->real_cap * sizeof(float), buf + nout * K - hp, c->real_cap * sizeof(float),
+			                     (hp + rem) * sizeof(float), c->cfg.nstreams, cudaMemcpyDeviceToDevice, c->s_comp));
 		}
 		CU(cudaEventRecord(c->ev_real_free[b], c->s_comp));
 		c->real_used[b] = true;
@@ -961,12 +1032,16 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_CS16IQ || nch != c->cfg.nch) return fail(ACB_ERR_ARG, "not a CS16 context / nch mismatch");
-	if (c->taps != c->cfg.K) return fail(ACB_ERR_ARG, "taps != K: supply the tables with acb_set_wf");
+	if (c->taps < c->cfg.K) return fail(ACB_ERR_ARG, "taps < K: supply the tables with acb_set_wf");
 	if (variant != ACB_CS16_SOAPY && variant != ACB_CS16_SDRPLAY) return fail(ACB_ERR_ARG, "unknown CS16 variant");
 	const unsigned fc = fc_hz ? fc_hz : acb_choose_fc(freqs_hz, nch, c->cfg.K);      /* soapy.c:132-136, sdrplay.c:124 */
 	if (fc == 0) return fail(ACB_ERR_PLAN, "Frequencies too far apart");
-	std::vector<float> wf((size_t)nch * c->cfg.K * 2);
-	for (int ch = 0; ch < nch; ch++) acb_cs16_build_wf(variant, freqs_hz[ch], fc, c->cfg.K, &wf[(size_t)ch * c->cfg.K * 2]);
+	const int T = c->taps;
+	std::vector<float> wf((size_t)nch * T * 2);
+	for (int ch = 0; ch < nch; ch++) {
+		if (c->hpad) acb_cs16_build_wf_lp(variant, freqs_hz[ch], fc, c->cfg.K, T, &wf[(size_t)ch * T * 2]);
+		else acb_cs16_build_wf(variant, freqs_hz[ch], fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
+	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
 	if (!c->fast) return ACB_OK;
@@ -980,13 +1055,17 @@ extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_F32REAL || nch != c->cfg.nch) return fail(ACB_ERR_ARG, "not a real-input context / nch mismatch");
-	if (c->taps != c->cfg.K) return fail(ACB_ERR_ARG, "taps != K: supply the tables with acb_set_wf");
+	if (c->taps < c->cfg.K) return fail(ACB_ERR_ARG, "taps < K: supply the tables with acb_set_wf");
 	unsigned lo = freqs_hz[0], hi = freqs_hz[0];
 	for (int i = 1; i < nch; i++) { lo = std::min(lo, freqs_hz[i]); hi = std::max(hi, freqs_hz[i]); }
 	const unsigned rate = (unsigned)c->cfg.K * ACB_INTRATE;
 	const unsigned fc = acb_air_choose_fc(lo, hi);
-	std::vector<float> wf((size_t)nch * c->cfg.K * 2);
-	for (int ch = 0; ch < nch; ch++) acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, &wf[(size_t)ch * c->cfg.K * 2]);
+	const int T = c->taps;
+	std::vector<float> wf((size_t)nch * T * 2);
+	for (int ch = 0; ch < nch; ch++) {
+		if (c->hpad) acb_air_build_wf_lp((int)freqs_hz[ch], (int)fc, rate, T, &wf[(size_t)ch * T * 2]);
+		else acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, &wf[(size_t)ch * T * 2]);
+	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
 	if (!c->fast) return ACB_OK;

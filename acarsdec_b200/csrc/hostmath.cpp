@@ -189,6 +189,75 @@ extern "C" void acb_cs16_build_wf(int variant, unsigned freq_hz, unsigned fc_hz,
 	}
 }
 
+/* ------------------------------------------------------------------ overlapping-window channel filter (taps > K) */
+
+/* modified Bessel function of the first kind, order 0: its power series, to the last double bit for the small
+ * arguments a Kaiser window needs (|x| <= beta = 6: terms fall below 1e-17 of the sum after ~25 of them) */
+static double bessel_i0(double x)
+{
+	const double q = x * x / 4;
+	double term = 1, sum = 1;
+	for (int k = 1; k < 200 && term > sum * 1e-18; k++) {
+		term *= q / ((double)k * k);
+		sum += term;
+	}
+	return sum;
+}
+
+extern "C" int acb_build_lowpass(int K, int taps, float *h)
+{
+	if (!h || K < 1 || taps < 1 || taps > ACB_MAXTAPS_PER_K * K) return ACB_ERR_ARG;
+	const double beta = 6.0, fcut = 0.5 / K;          /* cutoff in cycles per input sample: ACB_INTRATE/2 */
+	const double mid = (taps - 1) / 2.0, i0b = bessel_i0(beta);
+	std::vector<double> v(taps);
+	double sum = 0;
+	for (int n = 0; n < taps; n++) {
+		const double t = n - mid, x = 2 * fcut * t;
+		const double ideal = t == 0 ? 2 * fcut : 2 * fcut * sin(M_PI * x) / (M_PI * x);
+		const double r = taps > 1 ? 2.0 * n / (taps - 1) - 1 : 0;
+		v[n] = ideal * bessel_i0(beta * sqrt(std::max(0.0, 1 - r * r))) / i0b;
+		sum += v[n];
+	}
+	for (int n = 0; n < taps; n++) h[n] = (float)(v[n] / sum);
+	return ACB_OK;
+}
+
+/* w[i] = h[i] * exp(-j*2*pi*off*(i - H)/rate) * scale, off a whole number of Hz: the phase is reduced exactly in
+ * integers, then evaluated and multiplied in double and rounded to float once */
+static void build_wf_lp(long long off, long long rate, int K, int taps, double scale, float *wf)
+{
+	std::vector<float> h(taps);
+	acb_build_lowpass(K, taps, h.data());
+	const int H = taps - K;
+	for (int i = 0; i < taps; i++) {
+		const long long r = (off * (long long)(i - H)) % rate;
+		const double ph = 2.0 * M_PI * (double)r / (double)rate;
+		wf[2 * i] = (float)((double)h[i] * cos(ph) * scale);
+		wf[2 * i + 1] = (float)(-(double)h[i] * sin(ph) * scale);
+	}
+}
+
+extern "C" void acb_build_wf_lp(int fr_stored, unsigned fc_hz, int K, int taps, float *wf)
+{
+	/* rtl.c:283: the offset is the float image of the stored Fr minus the float image of Fc (both whole numbers) */
+	const float off = (float)fr_stored - (float)fc_hz;
+	build_wf_lp((long long)off, (long long)ACB_INTRATE * K, K, taps, 1.0 / 127.5, wf);
+}
+
+extern "C" void acb_cs16_build_wf_lp(int variant, unsigned freq_hz, unsigned fc_hz, int K, int taps, float *wf)
+{
+	/* soapy.c:159-162 / sdrplay.c:133-137: (float)Fr - (float)Fc; soapy.c:242's /32768.0 or sdrplay.c:225's /4 folded in */
+	const float off = (float)freq_hz - (float)fc_hz;
+	build_wf_lp((long long)off, (long long)ACB_INTRATE * K, K, taps, variant == ACB_CS16_SOAPY ? 1.0 / 32768.0 : 0.25, wf);
+}
+
+extern "C" void acb_air_build_wf_lp(int fr_hz, int fc_hz, unsigned rate, int taps, float *wf)
+{
+	/* air.c:263-285: the IF of the channel, Fc - Fr + rate/4 */
+	const unsigned K = rate / ACB_INTRATE;
+	build_wf_lp((long long)(unsigned)(fc_hz - fr_hz + rate / 4), (long long)rate, (int)K, taps, 1.0, wf);
+}
+
 extern "C" int acb_fast_plan(const unsigned *freqs_hz, int nch, int K, unsigned fc_hz, int *k_out, float *tw)
 {
 	/* The reference's table wf[ind] = cexpf(-j*AMFreq*ind)/K/127.5 (rtl.c:283-286) is a sampled complex

@@ -140,17 +140,22 @@ __device__ __forceinline__ void rmac(float2 &acc, float sv, const float2 w)
 	acc = fadd2_rn(acc, make_float2(__fmul_rn(w.x, sv), __fmul_rn(w.y, sv)));
 }
 
-template <int MODE>
+/* OVL (taps > K, DESIGN.md §4 "K1, overlapping window"): the window of a row starts `hbytes` (H_pad samples) before
+ * the row and is `taps` (= K + H_pad) samples long.  A 16-byte unit that lies before the stream's input of this submit
+ * is fetched from the history of the stream instead: `hist + s*hist_stride + hbytes` is where sample 0 of the submit
+ * would sit if the history were laid out in front of it.  The choice is per unit: H_pad and every row are whole units. */
+template <int MODE, bool OVL>
 __global__ void __launch_bounds__(CH_TILE)
 k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ wf,
-              float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp)
+              float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp,
+              const uint8_t *__restrict__ hist, size_t hist_stride, int hbytes)
 {
 	using T = C2<MODE>;
 	extern __shared__ __align__(16) unsigned char smem[];
 	const int t = threadIdx.x;
 	const int blk = blockIdx.x, s = blockIdx.y;
 	const size_t rowbytes = (size_t)K * T::TAP_BYTES;
-	const int U = taps * T::TAP_BYTES / 16;                          /* units of each row that carry taps (taps <= K) */
+	const int U = taps * T::TAP_BYTES / 16;                          /* units of each row's window that carry taps */
 	const int nchunk = (U + T::UNITS - 1) / T::UNITS;
 	const uint8_t *src_blk = in + (size_t)s * stream_stride + (size_t)blk * OUTBLK * rowbytes;
 	constexpr int NTILE = OUTBLK / C2_ROWS;
@@ -165,6 +170,7 @@ k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t
 			unsigned char *st = smem + (size_t)(step % T::STAGES) * T::STAGE_BYTES;
 			const int uc = min(T::UNITS, U - ck * T::UNITS);         /* units of this chunk */
 			const uint8_t *tsrc = src_blk + (size_t)tile * C2_ROWS * rowbytes + (size_t)ck * T::UNITS * 16;
+			if constexpr (OVL) tsrc -= hbytes;
 			{
 				/* unit u = t + 128*i of the chunk tile lives at (row u/uc, column u%uc): one division
 				 * per chunk, then incremental (the address arithmetic is a fifth of the kernel's
@@ -176,7 +182,12 @@ k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t
 				const size_t dstep = ((size_t)drow * T::ROW_UNITS + dj) * 16, sstep = (size_t)drow * rowbytes + (size_t)dj * 16;
 				const size_t dwrap = (size_t)(T::ROW_UNITS - uc) * 16, swrap = rowbytes - (size_t)uc * 16;
 				for (int u = t; u < C2_ROWS * uc; u += CH_TILE) {
-					cp_async16(dst, src);
+					if constexpr (OVL) {
+						const uint8_t *sbase = in + (size_t)s * stream_stride;
+						cp_async16(dst, src < sbase ? hist + (size_t)s * hist_stride + hbytes - (sbase - src) : src);
+					} else {
+						cp_async16(dst, src);
+					}
 					dst += dstep; src += sstep; j += dj;
 					if (j >= uc) { j -= uc; dst += dwrap; src += swrap; }
 				}
@@ -281,9 +292,11 @@ k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t
  * halve the table traffic per MAC; same arithmetic, same order, bit-identical results. */
 constexpr int R4_THREADS = 64, R4_RPT = C2_ROWS / R4_THREADS;
 
+template <bool OVL>                                                  /* OVL: as in k_channelize */
 __global__ void __launch_bounds__(R4_THREADS)
 k_channelize_real4(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ wf,
-                   float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp)
+                   float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp,
+                   const uint8_t *__restrict__ hist, size_t hist_stride, int hbytes)
 {
 	constexpr int UNITS = 5, TAPS_PER_UNIT = 4, W_BYTES = 8, CHUNK_TAPS = UNITS * TAPS_PER_UNIT, STAGES = 2;
 	constexpr int TILE_BYTES = C2_ROWS * UNITS * 16, STAGE_BYTES = TILE_BYTES + CHUNK_TAPS * CH_GROUP * W_BYTES;
@@ -303,6 +316,7 @@ k_channelize_real4(const uint8_t *__restrict__ in, size_t stream_stride, const u
 		unsigned char *st = smem + (size_t)(step % STAGES) * STAGE_BYTES;
 		const int uc = min(UNITS, U - ck * UNITS);
 		const uint8_t *tsrc = src_blk + (size_t)tile * C2_ROWS * rowbytes + (size_t)ck * UNITS * 16;
+		if constexpr (OVL) tsrc -= hbytes;
 		int row = t / uc, j = t - row * uc;
 		const int drow = R4_THREADS / uc, dj = R4_THREADS - drow * uc;
 		unsigned char *dst = st + ((size_t)row * UNITS + j) * 16;
@@ -310,7 +324,12 @@ k_channelize_real4(const uint8_t *__restrict__ in, size_t stream_stride, const u
 		const size_t dstep = ((size_t)drow * UNITS + dj) * 16, sstep = (size_t)drow * rowbytes + (size_t)dj * 16;
 		const size_t dwrap = (size_t)(UNITS - uc) * 16, swrap = rowbytes - (size_t)uc * 16;
 		for (int u = t; u < C2_ROWS * uc; u += R4_THREADS) {
-			cp_async16(dst, src);
+			if constexpr (OVL) {
+				const uint8_t *sbase = in + (size_t)s * stream_stride;
+				cp_async16(dst, src < sbase ? hist + (size_t)s * hist_stride + hbytes - (sbase - src) : src);
+			} else {
+				cp_async16(dst, src);
+			}
 			dst += dstep; src += sstep; j += dj;
 			if (j >= uc) { j -= uc; dst += dwrap; src += swrap; }
 		}
@@ -375,19 +394,21 @@ k_channelize_real4(const uint8_t *__restrict__ in, size_t stream_stride, const u
 	}
 }
 
+template <bool OVL>
 static int launch_channelize_real4(const void *in, size_t stream_stride, const void *wf, float *dm,
-                                   int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, cudaStream_t stream)
+                                   int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
 {
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	const size_t smem = 2 * (size_t)(C2_ROWS * 5 * 16 + 20 * CH_GROUP * 8);
-	cudaError_t e = cudaFuncSetAttribute(k_channelize_real4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	cudaError_t e = cudaFuncSetAttribute(k_channelize_real4<OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(k_channelize_real4, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	e = cudaFuncSetAttribute(k_channelize_real4<OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 	if (e != cudaSuccess) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
-	k_channelize_real4<<<grid, R4_THREADS, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
-	                                                      reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp);
+	k_channelize_real4<OVL><<<grid, R4_THREADS, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
+	                                                           reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
+	                                                           reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad * 4);
 	return (int)cudaGetLastError();
 }
 
@@ -398,39 +419,49 @@ size_t channelize_smem_bytes(int mode)
 	                           : (size_t)C2<IN_U8IQ>::STAGES * C2<IN_U8IQ>::STAGE_BYTES;
 }
 
-template <int MODE>
+template <int MODE, bool OVL>
 static int launch_channelize_t(const void *in, size_t stream_stride, const void *wf, float *dm,
-                               int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, cudaStream_t stream)
+                               int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
 {
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	const size_t smem = (size_t)C2<MODE>::STAGES * C2<MODE>::STAGE_BYTES;
-	cudaError_t e = cudaFuncSetAttribute(k_channelize<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	cudaError_t e = cudaFuncSetAttribute(k_channelize<MODE, OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) return (int)e;
 	/* both kernels ask for the largest shared-memory carve-out: an SM's L1/shared split only
 	 * changes when the SM is idle, so kernels that prefer different splits cannot be co-resident
 	 * — and the demod of submit i is meant to run underneath the channelizer of submit i+1 */
-	e = cudaFuncSetAttribute(k_channelize<MODE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	e = cudaFuncSetAttribute(k_channelize<MODE, OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 	if (e != cudaSuccess) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
-	k_channelize<MODE><<<grid, CH_TILE, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
-	                                                    reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp);
+	k_channelize<MODE, OVL><<<grid, CH_TILE, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
+	                                                         reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
+	                                                         reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad * C2<MODE>::TAP_BYTES);
 	return (int)cudaGetLastError();
 }
 
-/* whole 1024-row blocks of any input kind; the caller sends remaining rows to the generic kernel */
-int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
-                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, cudaStream_t stream)
+template <bool OVL>
+static int launch_channelize_k(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
+                               int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
 {
 	switch (mode) {
 	case IN_F32REAL: {
 		const bool two_rows = getenv("ACB_REAL_ROWS") && atoi(getenv("ACB_REAL_ROWS")) == 2;     /* A/B switch: the 2-rows-per-thread form */
-		return two_rows ? launch_channelize_t<IN_F32REAL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, stream)
-		                : launch_channelize_real4(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, stream);
+		return two_rows ? launch_channelize_t<IN_F32REAL, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream)
+		                : launch_channelize_real4<OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
 	}
-	case IN_CS16IQ: return launch_channelize_t<IN_CS16IQ>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, stream);
-	default: return launch_channelize_t<IN_U8IQ>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, stream);
+	case IN_CS16IQ: return launch_channelize_t<IN_CS16IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
+	default: return launch_channelize_t<IN_U8IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
 	}
+}
+
+/* whole 1024-row blocks of any input kind; the caller sends remaining rows to the generic kernel.  h.hpad > 0 selects
+ * the overlapping-window instantiations (taps = K + h.hpad) */
+int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
+                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
+{
+	return h.hpad ? launch_channelize_k<true>(mode, in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream)
+	              : launch_channelize_k<false>(mode, in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
 }
 
 /* ------------------------------------------------------------------------------------------
@@ -1358,6 +1389,76 @@ int launch_channelize_generic(int mode, const void *in, size_t stream_stride, co
 	if (mode == IN_F32REAL) k_channelize_generic<IN_F32REAL><<<grid, 128, 0, stream>>>(i8, stream_stride, w8, dm, K, taps, nch, ngrp, row0, nrows, nsamp);
 	else if (mode == IN_CS16IQ) k_channelize_generic<IN_CS16IQ><<<grid, 128, 0, stream>>>(i8, stream_stride, w8, dm, K, taps, nch, ngrp, row0, nrows, nsamp);
 	else k_channelize_generic<IN_U8IQ><<<grid, 128, 0, stream>>>(i8, stream_stride, w8, dm, K, taps, nch, ngrp, row0, nrows, nsamp);
+	return (int)cudaGetLastError();
+}
+
+/* The generic kernel's overlapping-window form (taps = K + hpad > K): tap i of row m reads sample m*K - hpad + i of the
+ * submit, from the stream's history when that index is negative.  Taps whose sample precedes the start of the stream
+ * (absolute row pos0 + m, counted from acb_create / acb_reset) are omitted, as the definition says; this is also the
+ * path that gives the u8 pipeline kernel's first rows after a reset their exact value (a raw zero byte of u8 history
+ * would convert to -127.37, not to 0). */
+template <int MODE>
+__global__ void __launch_bounds__(128)
+k_channelize_generic_ovl(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ wf,
+                         float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t row0, size_t nrows, size_t nsamp,
+                         const uint8_t *__restrict__ hist, size_t hist_stride, int hpad, unsigned long long pos0)
+{
+	constexpr int TB = MODE == IN_U8IQ ? 2 : 4;                      /* input bytes per sample */
+	const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const int s = blockIdx.y;
+	if (gid >= nrows * nch) return;
+	const size_t m = row0 + gid / nch;
+	const int ch = (int)(gid % nch);
+	const uint8_t *p = in + (size_t)s * stream_stride, *hp = hist + (size_t)s * hist_stride + (size_t)hpad * TB;
+	const long long o0 = (long long)m * K - hpad;                    /* sample of tap 0, relative to the submit */
+	const long long a0 = (long long)(pos0 + m) * K - hpad;           /* the same, counted from the stream start */
+	const int first = a0 < 0 ? (int)-a0 : 0;
+	float dr = 0.f, di = 0.f;
+	if (MODE == IN_F32REAL) {
+		const float2 *w = reinterpret_cast<const float2 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
+		for (int i = first; i < taps; i++) {
+			const long long o = o0 + i;
+			const float x = *reinterpret_cast<const float *>(o < 0 ? hp + o * TB : p + o * TB);
+			const float2 ww = w[(size_t)i * CH_GROUP];
+			dr = __fadd_rn(dr, __fmul_rn(ww.x, x));
+			di = __fadd_rn(di, __fmul_rn(ww.y, x));
+		}
+	} else {
+		const float4 *w = reinterpret_cast<const float4 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
+		for (int i = first; i < taps; i++) {
+			const long long o = o0 + i;
+			const uint8_t *q = o < 0 ? hp + o * TB : p + o * TB;
+			float a, b;
+			if (MODE == IN_CS16IQ) {
+				a = (float)reinterpret_cast<const short *>(q)[0];
+				b = (float)reinterpret_cast<const short *>(q)[1];
+			} else {
+				a = __fadd_rn((float)q[0], -127.37f);
+				b = __fadd_rn((float)q[1], -127.37f);
+			}
+			const float4 ww = w[(size_t)i * CH_GROUP];
+			dr = __fadd_rn(dr, __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, ww.z)));
+			di = __fadd_rn(di, __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.w)));
+		}
+	}
+	dm[((size_t)s * nsamp + m) * nch + ch] = envelope(make_float2(dr, di));
+}
+
+int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
+                                  int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
+                                  const Hist &h, cudaStream_t stream)
+{
+	if (nrows == 0) return 0;
+	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
+	const size_t total = nrows * nch;
+	dim3 grid((unsigned)((total + 127) / 128), nstreams);
+	const uint8_t *i8 = (const uint8_t *)in, *w8 = (const uint8_t *)wf, *h8 = (const uint8_t *)h.base;
+#define ACB_GEN_OVL(M) k_channelize_generic_ovl<M><<<grid, 128, 0, stream>>>(i8, stream_stride, w8, dm, K, taps, nch, ngrp, row0, nrows, nsamp, \
+	                                                                         h8, h.stride, h.hpad, h.pos0)
+	if (mode == IN_F32REAL) ACB_GEN_OVL(IN_F32REAL);
+	else if (mode == IN_CS16IQ) ACB_GEN_OVL(IN_CS16IQ);
+	else ACB_GEN_OVL(IN_U8IQ);
+#undef ACB_GEN_OVL
 	return (int)cudaGetLastError();
 }
 

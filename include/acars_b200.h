@@ -51,8 +51,21 @@ typedef struct {
 	int taps;               /* FIR length per output: 0 = K (the reference: boxcar x NCO over the whole
 	                           decimation period, rtl.c:283-286).  1..K selects the generalised case of
 	                           BASELINE configs 3/5: only the first `taps` samples of every K-sample row
-	                           are weighted (tables from acb_set_wf, nch x 2*taps floats), same arithmetic */
+	                           are weighted (tables from acb_set_wf, nch x 2*taps floats), same arithmetic.
+	                           K < taps <= ACB_MAXTAPS_PER_K*K: an overlapping window (a real channel filter, see
+	                           acb_build_lowpass), any input kind.  With H = taps - K, output row m (counted from
+	                           acb_create / acb_reset) is
+	                             dm[m] = | sum_{i<taps} x[m*K - H + i] * w[i] |
+	                           with x the front-end's converted sample ((float)u8 - 127.37f, (float)int16, the float
+	                           itself), the same rounded operations in ascending tap order, and the terms whose
+	                           sample index is negative omitted.  Row m still completes with sample (m+1)*K - 1, so
+	                           pos / block / soh_pos and the emission groups keep their meaning; the filter's extra
+	                           group delay of about (taps - K)/(2K) output samples is not compensated.  The context
+	                           keeps each stream's last H samples (rounded up to 16 bytes) across submits; acb_reset
+	                           clears them.  ACB_FLAG_FAST_CHANNELIZER is accepted and the exact kernel runs. */
 } acb_config_t;
+
+#define ACB_MAXTAPS_PER_K 16          /* longest overlapping window, in decimation periods */
 
 #define ACB_FLAG_NO_INPUT_STAGING 1   /* caller only uses acb_submit_device / acb_submit_dm_* */
 #define ACB_FLAG_CS16_INPUT 4         /* SoapySDR / SDRplay front-ends (soapy.c, sdrplay.c): int16 I,Q samples;
@@ -177,6 +190,20 @@ int acb_fast_plan_cs16(int variant, const unsigned *freqs_hz, int nch, int K, un
 int acb_fast_plan_air(const unsigned *freqs_hz, int nch, int K, unsigned fc_hz, int *k_out, float *tw);
 /* msk.c:44-48 — 133-tap oversampled half-cosine matched filter */
 void acb_build_h(float *h);
+/* Channel filter prototype for K < taps <= ACB_MAXTAPS_PER_K*K (no reference counterpart): an ideal low-pass with cutoff
+ * ACB_INTRATE/2 (1/(2K) of the input rate) centred at (taps-1)/2, times a Kaiser window with beta = 6.0, normalised to
+ * sum 1 in double and stored as float.  Returns ACB_OK, or ACB_ERR_ARG for K < 1 or taps outside 1..ACB_MAXTAPS_PER_K*K. */
+int acb_build_lowpass(int K, int taps, float *h);
+/* The planners' tables for taps > K (2*taps floats, re/im): w[i] = h[i] * mixer(i - H) * scale with h from
+ * acb_build_lowpass and H = taps - K, so tap i meets sample m*K - H + i of row m.  Each front-end's own mixer: the float
+ * images of the stored Fr and of Fc (rtl.c:283) and /127.5 for u8; soapy.c / sdrplay.c with the folded power-of-two
+ * scale for CS16 (as acb_cs16_build_wf); air.c's IF at rate/4 for real input.  The offset is a whole number of Hz, so
+ * the phase 2*pi*(offset*n mod rate)/rate is reduced exactly and evaluated in double (a float phase product, as the
+ * reference's K-tap tables use, would be off by up to 1/128 rad at 16K taps); each weight is rounded to float once.
+ * A carrier at the channel centre gives the reference's envelope level. */
+void acb_build_wf_lp(int fr_stored, unsigned fc_hz, int K, int taps, float *wf);
+void acb_cs16_build_wf_lp(int variant, unsigned freq_hz, unsigned fc_hz, int K, int taps, float *wf);
+void acb_air_build_wf_lp(int fr_hz, int fc_hz, unsigned rate, int taps, float *wf);
 
 /* ---- context ---- */
 
@@ -196,7 +223,9 @@ int acb_set_plan_air(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int n
 /* The channel part of initSoapy (soapy.c:112-163) / initSdrplay (sdrplay.c:95-138) for a CS16
  * context; fc_hz = 0 lets chooseFc pick the centre (soapy.c:132-133 honours a user frequency). */
 int acb_set_plan_cs16(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, int variant, unsigned fc_hz, unsigned *fc_out);
-/* Same, with caller-supplied tables (nch x 2K floats), e.g. taken from channel[].wf. */
+/* The planners (acb_set_plan, _at, _air, _cs16, and acb_multi_set_plan) build K-tap reference tables at taps = K and
+ * the acb_build_wf_lp family's low-pass tables at taps > K; they fail with ACB_ERR_ARG at taps < K.
+ * Same, with caller-supplied tables (nch x 2*taps floats; taps = K: e.g. taken from channel[].wf). */
 int acb_set_wf(acb_ctx_t *ctx, int stream, const float *wf, int nch);
 /* initMsk + initAcars for every channel of every stream (msk.c:30-51, acars.c:230-234). */
 int acb_reset(acb_ctx_t *ctx);
@@ -271,6 +300,8 @@ int   acb_copy_to_device(acb_ctx_t *ctx, void *dst_dev, const void *src_host, si
  * ACB_FLAG_FAST_CHANNELIZER: messages identical, intermediates as documented in DESIGN.md §2. */
 /* Envelope samples the channelizer produced for the last submit: out[(s*nsamp+n)*nch + c]. */
 int acb_read_dm(acb_ctx_t *ctx, float *out, size_t nfloats);
+/* The state is the demodulator's and the frame synchroniser's only: a round trip does not carry the channelizer's input
+ * side — the streaming front-ends' carried remainder, or the window history of a taps > K context. */
 int acb_get_state(acb_ctx_t *ctx, int stream, int chn, acb_chan_state_t *out);
 int acb_set_state(acb_ctx_t *ctx, int stream, int chn, const acb_chan_state_t *in);
 
