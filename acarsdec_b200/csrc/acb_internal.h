@@ -85,6 +85,8 @@ int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw,
                           int K, int nch, int nstreams, int nblk, size_t nsamp, bool fold8, CUstream_st *stream);
 int launch_channelize_dft_cs16(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
                                int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
+int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
+                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 bool channelize_rdft_supports(int K);
 int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
                            int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);

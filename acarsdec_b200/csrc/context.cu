@@ -89,6 +89,8 @@ struct acb_ctx {
 	int next_buf;
 	float *d_wf4;                /* [stream][grp][K][8] float4 (c, d, -d, c) */
 	bool fast;                   /* ACB_FLAG_FAST_CHANNELIZER and a shape k_channelize_dft takes */
+	bool fast_ovl;               /* ACB_FLAG_FAST_FILTER, taps > K, u8 / CS16 and a K k_channelize_ovl_fast takes */
+	float *d_p;                  /* fast_ovl: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
 	bool fold8;                  /* fast form: fold the row in half first (8-way split, K/8 MACs per channel) */
 	int demod_lanes;             /* lanes per channel in k_demod: 8 for small contexts, else 4 */
 	float *d_tw;                 /* fast form: [stream][grp][8 ch][K/4] (Tr, Ti) twiddles */
@@ -343,6 +345,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	CU(cudaStreamSynchronize(c->s_copy));
 	c->fast = (cfg->flags & ACB_FLAG_FAST_CHANNELIZER) && c->taps == cfg->K &&
 	          (c->in_kind == IN_KIND_F32REAL ? channelize_rdft_supports(cfg->K) : channelize_dft_supports(cfg->K));
+	c->fast_ovl = (cfg->flags & ACB_FLAG_FAST_FILTER) && c->taps > cfg->K && c->in_kind != IN_KIND_F32REAL &&
+	              channelize_dft_supports(cfg->K);
+	c->d_p = nullptr;
 	c->fast_ok.assign(cfg->nstreams, 0);
 	c->fold8 = true;             /* K/8 instead of K/4 MACs per channel than the plain 4-way split */
 	if (const char *e = getenv("ACB_FAST_FOLD8")) c->fold8 = atoi(e) != 0;          /* comparison switch; both are tested */
@@ -358,9 +363,18 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 			if (v == -4 || v == -8 || (v > 0 && v < 64 && (l == 1 || l == 2 || l == 4 || l == 8))) c->demod_lanes = v;
 		}
 	}
-	if (c->fast) {
+	if (c->fast || c->fast_ovl) {
 		CU(cudaMalloc(&c->d_tw, (size_t)cfg->nstreams * c->ngrp * CH_GROUP * (cfg->K / 4) * 2 * sizeof(float)));
 		CU(cudaMalloc(&c->d_twmeta, (size_t)cfg->nstreams * c->ngrp * sizeof(unsigned)));
+	}
+	if (c->fast_ovl) {
+		/* the polyphase weights p[i] = fl(K * h[i]), laid out like the exact table (taps_pad entries, the hpad - H in front
+		 * zero): the same for every channel and stream; with the twiddles' 1/K the pre-sum's bin carries h[i] * scale */
+		std::vector<float> h(c->taps), p(c->taps_pad, 0.0f);
+		acb_build_lowpass(cfg->K, c->taps, h.data());
+		for (int i = 0; i < c->taps; i++) p[c->taps_pad - c->taps + i] = (float)cfg->K * h[i];
+		CU(cudaMalloc(&c->d_p, p.size() * sizeof(float)));
+		if (int r = upload(c, c->d_p, p.data(), p.size() * sizeof(float))) return r;
 	}
 	c->dm_floats = (size_t)cfg->nstreams * cfg->max_blocks * OUTBLK * cfg->nch;
 	for (int i = 0; i < NPIPE; i++) {
@@ -429,7 +443,7 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 		cudaFree(c->d_planar);
 		cudaFree(c->d_hist);
 		cudaFree(c->d_wf4); cudaFree(c->d_state);
-		cudaFree(c->d_tw); cudaFree(c->d_twmeta);
+		cudaFree(c->d_tw); cudaFree(c->d_twmeta); cudaFree(c->d_p);
 		for (int i = 0; i < NPIPE; i++) {
 			cudaFree(c->d_dm[i]); cudaEventDestroy(c->ev_k1_done[i]); cudaEventDestroy(c->ev_dm_free[i]);
 			cudaEventDestroy(c->ev_k2_done[i]); cudaEventDestroy(c->ev_ring_read[i]);
@@ -522,8 +536,9 @@ extern "C" int acb_set_plan_at(acb_ctx_t *c, int stream, const unsigned *freqs_h
 		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
 	}
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	if (!c->fast) return ACB_OK;
-	/* Fast form: per-channel bin numbers and twiddles, when every channel sits on the raster */
+	if (!c->fast && !c->fast_ovl) return ACB_OK;
+	/* Fast forms (taps = K, or the overlapping window's polyphase form): per-channel bin numbers and twiddles, when every
+	 * channel sits on the raster */
 	const int K = c->cfg.K, N2 = K / 4;
 	std::vector<int> kbin(nch);
 	std::vector<float> tw1((size_t)nch * N2 * 2);
@@ -762,9 +777,10 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		/* whole 1024-row blocks through the pipeline kernel, the remaining rows (submits of 4-byte
 		 * samples may carry any count) and unaligned K through the generic one */
 		const int fast = c->use_generic ? 0 : nsamp / OUTBLK;
-		bool dft = c->fast;                         /* every stream planned on the raster? */
+		bool dft = c->fast || c->fast_ovl;           /* every stream planned on the raster? */
 		for (int s = 0; dft && s < c->cfg.nstreams; s++) dft = c->fast_ok[s] != 0;
 		bool all_rows = false;                       /* the fast CS16 kernel takes partial blocks too */
+		bool ovl_fast = false;                       /* the polyphase form ran: it omits the terms before the stream start itself */
 		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
 		 * for the streaming kinds (submit4) */
 		Hist hist{ nullptr, 0, c->hpad, c->pos };
@@ -775,7 +791,14 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			hist.base = d_iq - (size_t)c->hpad * 4;
 			hist.stride = stride;
 		}
-		if (dft && c->in_kind == IN_KIND_F32REAL && !c->use_generic) {
+		if (dft && c->fast_ovl) {
+			r = launch_channelize_ovl_fast(c->in_kind, d_iq, stride, hist, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			c->stats.kernel_launches++;
+			c->stats.fast_chan_launches++;
+			all_rows = true;
+			ovl_fast = true;
+		} else if (dft && c->in_kind == IN_KIND_F32REAL && !c->use_generic) {
 			r = launch_channelize_rdft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
 			c->stats.kernel_launches++;
 			c->stats.fast_chan_launches++;
@@ -808,7 +831,7 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			 * create / reset — are recomputed with those terms omitted */
 			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
 			const unsigned long long lead = (H + K - 1) / K;
-			if (!r && fast && c->pos < lead) {
+			if (!r && fast && !ovl_fast && c->pos < lead) {
 				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
 				                                  0, (size_t)std::min<unsigned long long>(lead - c->pos, (unsigned long long)nsamp), (size_t)nsamp,
 				                                  hist, c->s_comp);
@@ -1044,7 +1067,7 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	if (!c->fast) return ACB_OK;
+	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<int> kbin(nch);
 	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
 	const bool ok = acb_fast_plan_cs16(variant, freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;

@@ -1031,6 +1031,262 @@ static int launch_dft1_t(const uint8_t *in, size_t stream_stride, const float2 *
 }
 
 /* ------------------------------------------------------------------------------------------
+ * K1, overlapping window, polyphase fast form (ACB_FLAG_FAST_FILTER; DESIGN.md §4).  With every channel on the 12.5 kHz
+ * raster the low-pass table of a taps > K context is w[i] = h[i] * exp(-j*2*pi*k*(i - H)/K) * scale: one real prototype
+ * times a DFT exponential of period K.  Split the window of row m by the phase n = (i - H) mod K:
+ *
+ *     D = sum_{n < K} T[n] * z_m[n],   z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K],   p = fl(K * h),
+ *     T[n] = exp(-j*2*pi*k*n/K)/K * scale   (the twiddles of the boxcar fast form)
+ *
+ * z_m (the polyphase pre-sum) is shared by every channel of the stream; each channel then needs the bin of a K-point
+ * DFT of one row, which is k_channelize_dft1's fold / shared 4-point DFT / residue-sorted MAC columns unchanged.
+ *
+ * Shape: k_channelize_dft1's, with the window.  A warp's tile is its 32 rows plus the hpad samples in front of them (the
+ * halo, HR = ceil(hpad/K) more rows, the first one partial), staged by one bulk copy per row; rows before the submit come
+ * from the stream's history (u8: the context's buffer; CS16: the samples in front of the input), the same address rule as
+ * k_channelize<MODE, true>.  Lane l builds z of its row l from the staged window — for each 4-sample group of an eighth
+ * of the row, the terms r = rlo .. 0 in ascending tap order, one FFMA per component — folds and splits it in registers
+ * and hands it to the MAC columns: z never leaves the SM.  p (taps_pad floats, zero weights in front like the exact
+ * table) is read through L1 with a warp-uniform address.  Terms whose row lies before the stream start (absolute row
+ * pos0 + m + r < 0) are skipped, so the rows after acb_create / acb_reset need no second kernel: for u8 the zero bytes of
+ * a cleared history would convert to -127.37, not to 0.
+ *
+ * Zero-weight terms (the front padding of p) leave z exactly as it was: z starts at +0, fma(+0, x, +0) = +0, and once a
+ * real term has arrived, z + (+-0) = z.  So this kernel's z equals the restatement's sum over the valid terms only
+ * (tests/host/ovl_fast_oracle.c: orc_channelize_ovl_fast), bit for bit.
+ * ---------------------------------------------------------------------------------------- */
+template <int KIND, int UNITS, int WARPS>
+__global__ void __launch_bounds__(32 * WARPS)
+k_channelize_ovl_fast(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ hist, size_t hist_stride,
+                      int hpad, unsigned long long pos0, const float *__restrict__ pw, const float2 *__restrict__ tw,
+                      const unsigned *__restrict__ meta, float *__restrict__ dm, int nch, int ngrp, size_t nsamp)
+{
+	using P = Dft1Plan<KIND, UNITS, WARPS>;
+	constexpr int K = UNITS * 8, BPS = P::BPS;
+	constexpr int CU = UNITS / 4;                 /* groups of 4 samples per eighth of a row */
+	constexpr int N2 = P::N2;
+	constexpr int NTILE = OUTBLK / DFT1_ROWS;
+	extern __shared__ __align__(16) unsigned char smem[];
+	const int l = threadIdx.x & 31;
+	const int w = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+	const int blk = blockIdx.x, s = blockIdx.y, g = blockIdx.z;
+	const int HR = (hpad + K - 1) / K;            /* halo rows in front of the tile, the first one from sample n0 on */
+	const int n0 = HR * K - hpad;
+	/* rows one by one, each shifted by 16 more bytes (a lane's terms r, r+1 are one stride apart: one add per term) */
+	constexpr int STRIDE = P::ROWBYTES + 16;
+	const size_t tile_bytes = (size_t)(DFT1_ROWS + HR) * STRIDE;
+	unsigned char *mytile = smem + (size_t)w * tile_bytes;
+	const float4 *stw = reinterpret_cast<const float4 *>(smem + (size_t)WARPS * tile_bytes);     /* [slot][n2] (Tr, Ti) */
+	unsigned long long *bar = reinterpret_cast<unsigned long long *>(smem + (size_t)WARPS * tile_bytes + P::TW_BYTES) + w;
+	const uint8_t *src_s = in + (size_t)s * stream_stride;
+	const uint8_t *hist_s = hist + (size_t)s * hist_stride + (size_t)hpad * BPS;      /* where sample 0 of the submit would sit */
+	const unsigned m = __shfl_sync(0xffffffffu, meta[(size_t)s * ngrp + g], 0);
+
+	if (l == 0) mbar_init(bar, 1);
+	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+	/* channel slots sorted by residue (k_c / 2) mod 4, as in k_channelize_dft1 */
+	unsigned pperm = 0;
+	int bnd0, bnd1, bnd2;
+	{
+		int cnt[4] = { 0, 0, 0, 0 };
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) {
+			const unsigned r = (m >> (16 + 2 * c)) & 3u;
+#pragma unroll
+			for (int q = 0; q < 4; q++) cnt[q] += (r == (unsigned)q);
+		}
+		bnd0 = cnt[0]; bnd1 = bnd0 + cnt[1]; bnd2 = bnd1 + cnt[2];
+		int pos[4] = { 0, bnd0, bnd1, bnd2 };
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) {
+			const unsigned r = (m >> (16 + 2 * c)) & 3u;
+			int at = 0;
+#pragma unroll
+			for (int q = 0; q < 4; q++) { at = (r == (unsigned)q) ? pos[q] : at; pos[q] += (r == (unsigned)q); }
+			pperm |= (unsigned)c << (3 * at);
+		}
+	}
+	{
+		const uint4 *tsrc = reinterpret_cast<const uint4 *>(tw + ((size_t)s * ngrp + g) * N2 * CH_GROUP);
+		uint4 *tdst = reinterpret_cast<uint4 *>(smem + (size_t)WARPS * tile_bytes);
+		constexpr int PER = N2 * 8 / 16;
+		for (int q = threadIdx.x; q < P::TW_BYTES / 16; q += 32 * WARPS) {
+			const int j = q / PER, off = q - j * PER;
+			cp_async16(tdst + q, tsrc + ((pperm >> (3 * j)) & 7u) * PER + off);
+		}
+		cp_async_commit();
+		cp_async_wait_all();
+	}
+	__syncthreads();
+
+	const size_t rows_left = nsamp - (size_t)blk * OUTBLK;
+	const int tiles_here = rows_left >= (size_t)OUTBLK ? NTILE : (int)((rows_left + DFT1_ROWS - 1) / DFT1_ROWS);
+	const int ntile = (tiles_here - w + WARPS - 1) / WARPS;
+	auto issue = [&](int n) {
+		if (elect_one()) {
+			mbar_expect_tx(bar, (unsigned)((hpad + DFT1_ROWS * K) * BPS));
+			const long long row0 = (long long)blk * OUTBLK + (long long)(w + n * WARPS) * DFT1_ROWS - HR;
+			for (int b = 0; b < DFT1_ROWS + HR; b++) {
+				const int s0 = b == 0 ? n0 : 0;
+				const long long smp = (row0 + b) * K + s0;           /* >= -hpad: before the submit means in the history */
+				const uint8_t *src = smp < 0 ? hist_s + smp * BPS : src_s + smp * BPS;
+				bulk_g2s(mytile + (size_t)b * STRIDE + s0 * BPS, src, (unsigned)((K - s0) * BPS), bar);
+			}
+		}
+	};
+	if (ntile > 0) issue(0);
+	const int nc = min(CH_GROUP, nch - g * CH_GROUP);
+
+	for (int n = 0; n < ntile; n++) {
+		const int tile = w + n * WARPS;
+		mbar_wait(bar, (unsigned)(n & 1));
+		const size_t mrow = (size_t)blk * OUTBLK + (size_t)tile * DFT1_ROWS + l;
+		const unsigned long long mabs = pos0 + mrow;                  /* row counted from the stream start */
+		float2 A[CH_GROUP], B[CH_GROUP];
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) A[c] = B[c] = make_float2(0.f, 0.f);
+
+#pragma unroll 1
+		for (int g4 = 0; g4 < CU; g4++) {
+			/* the pre-sum z of samples n .. n+3 of eighth e, in ascending tap order */
+			auto presum = [&](int e, float2 (&z)[4]) {
+				const int nn = e * (K / 8) + 4 * g4;
+				int rlo = -((nn + hpad) / K);                            /* warp-uniform: the same for the 4 samples */
+				if ((unsigned long long)(-rlo) > mabs) rlo = -(int)mabs;  /* rows before the stream start: omitted */
+#pragma unroll
+				for (int k = 0; k < 4; k++) z[k] = make_float2(0.f, 0.f);
+				const float *pr = pw + nn + hpad;
+				const unsigned char *myrow = mytile + (size_t)(l + HR) * STRIDE + nn * BPS;
+#pragma unroll 2
+				for (int r = rlo; r <= 0; r++) {
+					const unsigned char *q = myrow + r * STRIDE;
+					const float4 pv = __ldg(reinterpret_cast<const float4 *>(pr + r * K));
+					const float pk[4] = { pv.x, pv.y, pv.z, pv.w };
+					float2 x[4];
+					if (KIND == IN_CS16IQ) {
+						const uint4 u = *reinterpret_cast<const uint4 *>(q);
+						x[0] = cvt_cs16(u.x); x[1] = cvt_cs16(u.y); x[2] = cvt_cs16(u.z); x[3] = cvt_cs16(u.w);
+					} else {
+						const uint2 u = *reinterpret_cast<const uint2 *>(q);
+						x[0] = cvt_iq(u.x, 0); x[1] = cvt_iq(u.x, 1); x[2] = cvt_iq(u.y, 0); x[3] = cvt_iq(u.y, 1);
+					}
+#pragma unroll
+					for (int k = 0; k < 4; k++) z[k] = ffma2(x[k], make_float2(pk[k], pk[k]), z[k]);
+				}
+			};
+			float2 Y[4][4];                       /* [residue][sample of the group] = (re, im) */
+#pragma unroll
+			for (int n1 = 0; n1 < 4; n1++) {      /* fold: z'[n] = z[n] + z[n + K/2], eighths n1 and n1 + 4 */
+				float2 za[4], zb[4];
+				presum(n1, za);
+				presum(n1 + 4, zb);
+#pragma unroll
+				for (int k = 0; k < 4; k++) Y[n1][k] = fadd2_rn(za[k], zb[k]);
+			}
+#pragma unroll
+			for (int k = 0; k < 4; k++) {
+				const float2 z0 = Y[0][k], z1 = Y[1][k], z2 = Y[2][k], z3 = Y[3][k];
+				const float2 s02 = fadd2_rn(z0, z2), s13 = fadd2_rn(z1, z3);
+				const float2 d02 = fsub2(z0, z2);
+				const float2 wj = make_float2(__fadd_rn(z1.y, -z3.y), __fadd_rn(z3.x, -z1.x));   /* -j (z1 - z3) */
+				Y[0][k] = fadd2_rn(s02, s13);
+				Y[2][k] = fsub2(s02, s13);
+				Y[1][k] = fadd2_rn(d02, wj);      /* (z0 - z2) - j (z1 - z3) */
+				Y[3][k] = fsub2(d02, wj);         /* (z0 - z2) + j (z1 - z3) */
+			}
+			const float4 *tj = stw + g4 * 2;
+			float4 nu0 = tj[0], nu1 = tj[1];
+#define ACB_OVF_MAC(J, R)                                                                  \
+			{                                                                                      \
+				const float4 u0 = nu0, u1 = nu1;                                                       \
+				if ((J) + 1 < CH_GROUP) { nu0 = tj[((J) + 1) * (N2 / 2)]; nu1 = tj[((J) + 1) * (N2 / 2) + 1]; } \
+				const float2 tt[4] = { make_float2(u0.x, u0.y), make_float2(u0.z, u0.w),               \
+				                       make_float2(u1.x, u1.y), make_float2(u1.z, u1.w) };             \
+				_Pragma("unroll") for (int k = 0; k < 4; k++) {                                        \
+					A[J] = ffma2(make_float2(Y[R][k].x, Y[R][k].x), tt[k], A[J]);                          \
+					B[J] = ffma2(make_float2(Y[R][k].y, Y[R][k].y), tt[k], B[J]);                          \
+				}                                                                                      \
+			}
+#define ACB_OVF_C0(J) if ((J) >= bnd0) goto c1_##J; ACB_OVF_MAC(J, 0)
+#define ACB_OVF_C1(J) c1_##J: if ((J) >= bnd1) goto c2_##J; ACB_OVF_MAC(J, 1)
+#define ACB_OVF_C2(J) c2_##J: if ((J) >= bnd2) goto c3_##J; ACB_OVF_MAC(J, 2)
+#define ACB_OVF_C3(J) c3_##J: ACB_OVF_MAC(J, 3)
+#define ACB_OVF_COL(C) C(0) C(1) C(2) C(3) C(4) C(5) C(6) C(7)
+			ACB_OVF_COL(ACB_OVF_C0) goto macs_done;
+			ACB_OVF_COL(ACB_OVF_C1) goto macs_done;
+			ACB_OVF_COL(ACB_OVF_C2) goto macs_done;
+			ACB_OVF_COL(ACB_OVF_C3)
+			macs_done:;
+#undef ACB_OVF_COL
+#undef ACB_OVF_C3
+#undef ACB_OVF_C2
+#undef ACB_OVF_C1
+#undef ACB_OVF_C0
+#undef ACB_OVF_MAC
+		}
+		/* every lane is done with the staged window: the buffer can take the warp's next tile */
+		__syncwarp();
+		if (n + 1 < ntile) issue(n + 1);
+		float e[CH_GROUP];
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) {
+			const float re = __fadd_rn(A[c].x, -B[c].y), im = __fadd_rn(A[c].y, B[c].x);
+			/* |D| in float, as k_channelize_dft1: integer input and a prototype of sum 1 bound it (u8: |D| <= ~1.5, CS16:
+			 * <= ~1.2e4 times the filter's peak gain, no overflow); the < 3e-23 absolute error of a denormal re*re is far
+			 * below 1e-6 of the row total sum |x| |w| of any row that is not all zeros */
+			e[c] = __fsqrt_rn(__fmaf_rn(re, re, __fmul_rn(im, im)));
+		}
+		float *o = dm + ((size_t)s * nsamp + mrow) * nch + g * CH_GROUP;
+#pragma unroll
+		for (int j = 0; j < CH_GROUP; j++) {
+			const int c = (int)((pperm >> (3 * j)) & 7u);
+			if (c < nc && mrow < nsamp) o[c] = e[j];
+		}
+	}
+}
+
+template <int KIND, int UNITS, int WARPS>
+static int launch_ovl_fast_t(const uint8_t *in, size_t stream_stride, const Hist &h, const float *p, const float2 *tw,
+                             const unsigned *meta, float *dm, int nch, int nstreams, int nblk, size_t nsamp, cudaStream_t stream)
+{
+	using P = Dft1Plan<KIND, UNITS, WARPS>;
+	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
+	const int HR = (h.hpad + UNITS * 8 - 1) / (UNITS * 8);
+	/* shared memory grows with the halo only: (32 + HR) rows per warp */
+	const int smem = WARPS * (DFT1_ROWS + HR) * (P::ROWBYTES + 16) + P::TW_BYTES + WARPS * 8;
+	auto kern = k_channelize_ovl_fast<KIND, UNITS, WARPS>;
+	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	if (e != cudaSuccess) return (int)e;
+	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	if (e != cudaSuccess) return (int)e;
+	dim3 grid(nblk, nstreams, ngrp);
+	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad, h.pos0,
+	                                         p, tw, meta, dm, nch, ngrp, nsamp);
+	return (int)cudaGetLastError();
+}
+
+/* u8 IQ or CS16 IQ, taps > K, K in {160, 192}, every channel on the 12.5 kHz raster; `nsamp` output rows per stream, any
+ * count (CS16: the input buffer carries 32 rows of slack); `p` = taps_pad floats, fl(K*h) behind hpad - H zeros */
+int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
+                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	if (nsamp == 0) return 0;
+	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
+	const float2 *t4 = reinterpret_cast<const float2 *>(tw);
+	const int nblk = (int)((nsamp + OUTBLK - 1) / OUTBLK);
+#define ACB_OVF_GO(M, U) launch_ovl_fast_t<M, U, 2>(i8, stream_stride, h, p, t4, meta, dm, nch, nstreams, nblk, nsamp, stream)
+	if (mode == IN_CS16IQ) {
+		if (K == 160) return ACB_OVF_GO(IN_CS16IQ, 20);
+		if (K == 192) return ACB_OVF_GO(IN_CS16IQ, 24);
+	} else if (mode == IN_U8IQ) {
+		if (K == 160) return ACB_OVF_GO(IN_U8IQ, 20);
+		if (K == 192) return ACB_OVF_GO(IN_U8IQ, 24);
+	}
+#undef ACB_OVF_GO
+	return (int)cudaErrorInvalidValue;
+}
+
+/* ------------------------------------------------------------------------------------------
  * Fast form of the REAL-input channelizer (air.c:291-341 with the table of air.c:278-285): wf[i] = exp(-j*2*pi*k*i/K)/K is
  * a sampled exponential with k = (Fc - Fr + rate/4) / 12.5 kHz a whole number whenever the channels and the tuner
  * centre sit on the 12.5 kHz raster (air.c:66 puts Fc there), so D is bin k of the K-point DFT of a REAL row:

@@ -62,7 +62,8 @@ typedef struct {
 	                           pos / block / soh_pos and the emission groups keep their meaning; the filter's extra
 	                           group delay of about (taps - K)/(2K) output samples is not compensated.  The context
 	                           keeps each stream's last H samples (rounded up to 16 bytes) across submits; acb_reset
-	                           clears them.  ACB_FLAG_FAST_CHANNELIZER is accepted and the exact kernel runs. */
+	                           clears them.  ACB_FLAG_FAST_CHANNELIZER is accepted and the exact kernel runs;
+                           ACB_FLAG_FAST_FILTER selects the polyphase fast form of this filter. */
 } acb_config_t;
 
 #define ACB_MAXTAPS_PER_K 16          /* longest overlapping window, in decimation periods */
@@ -80,6 +81,20 @@ typedef struct {
                                          order: relative to the total in-band signal the envelope is within 1e-6 of the exact DFT
                                          bin and within the reference's own table rounding (1e-5) of the reference; decoded
                                          messages are the same; without this flag the envelope is bit-identical */
+#define ACB_FLAG_FAST_FILTER 16        /* taps > K (the overlapping window) on u8 IQ contexts planned with acb_set_plan,
+                                         acb_set_plan_at or acb_multi_set_plan and CS16 contexts planned with
+                                         acb_set_plan_cs16, K = 160 or 192, every stream's channels on the 12.5 kHz raster
+                                         around Fc (as ACB_FLAG_FAST_CHANNELIZER decides it): the polyphase fast form.  The
+                                         window is pre-summed once per stream into one K-sample row per output,
+                                           z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K],  p = fl(K * h)  (h: acb_build_lowpass)
+                                         (ascending tap order, one FMA per term, terms before the stream start omitted), and
+                                         each channel's bin of that row is taken as the boxcar fast form takes it:
+                                         2*taps/K + ~7 FP32 lane-ops per complex sample instead of 8*C*taps/K.  NOT the
+                                         exact form's operation order: per output row, with S = sum |x|*|w|, the envelope is
+                                         within 1e-5*S of the exact form's and within 1e-6*S of the float64 definition;
+                                         decoded messages are the same.  Anything else (a stream off the raster, a table given
+                                         through acb_set_wf, another K, real input) runs the exact kernel, as does taps <= K,
+                                         where this flag has no effect. */
 #define ACB_FLAG_REAL_INPUT 2         /* Airspy front-end (air.c): float32 REAL samples at IF = rate/4,
                                          rate = K*12500; use acb_set_plan_air / acb_submit_real_host */
 
@@ -319,7 +334,8 @@ typedef struct {
 	double   chan_ms;           /* accumulated device time of the channelizer kernel (CUDA events) */
 	double   demod_ms;          /* accumulated device time from a demod kernel's start to the end of its block FEC */
 	uint64_t chan_launches, demod_launches;
-	uint64_t fast_chan_launches; /* channelizer launches that took the ACB_FLAG_FAST_CHANNELIZER form */
+	uint64_t fast_chan_launches; /* channelizer launches that took a fast form: ACB_FLAG_FAST_CHANNELIZER's (taps = K) or
+	                                ACB_FLAG_FAST_FILTER's (taps > K) */
 	uint64_t frames_lost;       /* frames that found the device ring full (ACB_ERR_OVERFLOW was returned once per submit) */
 	double   host_ms;           /* accumulated wall time the consumer thread spent ordering and queuing frames */
 } acb_stats_t;
