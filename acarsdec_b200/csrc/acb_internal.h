@@ -90,6 +90,8 @@ int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, c
 bool channelize_rdft_supports(int K);
 int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
                            int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
+int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
+                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
 int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_stride, uint32_t *out, size_t out_stride,
                            size_t nsamples, int nstreams, CUstream_st *stream);

@@ -89,7 +89,9 @@ struct acb_ctx {
 	int next_buf;
 	float *d_wf4;                /* [stream][grp][K][8] float4 (c, d, -d, c) */
 	bool fast;                   /* ACB_FLAG_FAST_CHANNELIZER and a shape k_channelize_dft takes */
-	bool fast_ovl;               /* ACB_FLAG_FAST_FILTER, taps > K, u8 / CS16 and a K k_channelize_ovl_fast takes */
+	bool fast_ovl;               /* taps > K and the polyphase form: ACB_FLAG_FAST_FILTER on u8 / CS16 with a K
+	                                k_channelize_ovl_fast takes, ACB_FLAG_FAST_FILTER_REAL on real input with a K
+	                                k_channelize_ovl_rdft takes */
 	float *d_p;                  /* fast_ovl: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
 	bool fold8;                  /* fast form: fold the row in half first (8-way split, K/8 MACs per channel) */
 	int demod_lanes;             /* lanes per channel in k_demod: 8 for small contexts, else 4 */
@@ -345,8 +347,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	CU(cudaStreamSynchronize(c->s_copy));
 	c->fast = (cfg->flags & ACB_FLAG_FAST_CHANNELIZER) && c->taps == cfg->K &&
 	          (c->in_kind == IN_KIND_F32REAL ? channelize_rdft_supports(cfg->K) : channelize_dft_supports(cfg->K));
-	c->fast_ovl = (cfg->flags & ACB_FLAG_FAST_FILTER) && c->taps > cfg->K && c->in_kind != IN_KIND_F32REAL &&
-	              channelize_dft_supports(cfg->K);
+	c->fast_ovl = c->taps > cfg->K &&
+	              (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_FILTER_REAL) && channelize_rdft_supports(cfg->K)
+	                                             : (cfg->flags & ACB_FLAG_FAST_FILTER) && channelize_dft_supports(cfg->K));
 	c->d_p = nullptr;
 	c->fast_ok.assign(cfg->nstreams, 0);
 	c->fold8 = true;             /* K/8 instead of K/4 MACs per channel than the plain 4-way split */
@@ -791,7 +794,14 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			hist.base = d_iq - (size_t)c->hpad * 4;
 			hist.stride = stride;
 		}
-		if (dft && c->fast_ovl) {
+		if (dft && c->fast_ovl && c->in_kind == IN_KIND_F32REAL) {
+			/* the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
+			r = launch_channelize_ovl_rdft(d_iq, stride, c->hpad, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			c->stats.kernel_launches++;
+			c->stats.fast_chan_launches++;
+			all_rows = true;
+		} else if (dft && c->fast_ovl) {
 			r = launch_channelize_ovl_fast(c->in_kind, d_iq, stride, hist, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
 			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
 			c->stats.kernel_launches++;
@@ -1091,7 +1101,7 @@ extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_
 	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	if (!c->fast) return ACB_OK;
+	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<int> kbin(nch);
 	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
 	const bool ok = acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;

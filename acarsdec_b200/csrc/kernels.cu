@@ -1512,6 +1512,293 @@ int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw
 	return (int)cudaErrorInvalidValue;
 }
 
+/* ------------------------------------------------------------------------------------------
+ * Polyphase fast form of the overlapping window for REAL input (ACB_FLAG_FAST_FILTER_REAL, taps > K): with every channel on
+ * the raster, w[i] = h[i] * exp(-j*2*pi*k*(i - H)/K), so D is bin k of the K-sample real row
+ *   z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K],   p = fl(K*h), r <= 0 ascending (ascending tap order), one FMA per term
+ * and that bin is taken exactly as k_channelize_rdft takes it from a row of input (the same lanes per row, n2-pair ranges,
+ * MAC columns and pairwise tree; twiddles from acb_fast_plan_air, which carry the 1/K).
+ *
+ * Shape: one CTA per (1024-row block, stream, channel group), as k_channelize_rdft.  The CTA walks its block in steps of
+ * T = WARPS * ROWS rows through a ring of HR + T staged rows (HR = ceil(hpad/K)): each input row is staged once per CTA
+ * and the halo once per block, so shared memory is (HR + T) rows, not a private (ROWS + HR)-row window per warp.  A step:
+ *  1. the next T rows arrive by bulk copies (the first step also brings the HR rows in front of the block, the first one
+ *     from sample n0 on: rows before the submit are the history right in front of the input in d_real);
+ *  2. the pre-sum: thread u owns the CW columns u*CW .. of every row, walks the step's rows four at a time (each staged
+ *     sample is read once for four rows; p is read through L1 once per term) and writes z_m over the slot of input row
+ *     m - HR, which no later row of this step reads: a thread only overwrites its own columns, and rows <= m are done;
+ *  3. the rdft's DFT half on the z rows, then the envelope in double;
+ *  4. the z slots are where the next step's rows land.
+ * Terms before the stream start READ the history, which acb_create / acb_reset zero: z starts at +0 and is never -0 (an
+ * exact zero sum rounds to +0), so fma(p, +0, z) = z, and the table's zero front padding gives fma(+0, x, +0) = +0 for
+ * the finite samples there.  The result is the sum over the valid terms only (tests/host/ovl_fast_real_oracle.c:
+ * orc_ovl_presum_real, then orc_channelize_rdft), bit for bit.  Every fetch lies in [-hpad, nsamp*K) samples of its
+ * stream: no slack rows are read.
+ * ---------------------------------------------------------------------------------------- */
+template <int CW> struct ColsF;
+template <> struct ColsF<2> {
+	static __device__ __forceinline__ void ld(const float *a, float (&v)[2]) { const float2 u = *reinterpret_cast<const float2 *>(a); v[0] = u.x; v[1] = u.y; }
+	static __device__ __forceinline__ void ldg(const float *a, float (&v)[2]) { const float2 u = __ldg(reinterpret_cast<const float2 *>(a)); v[0] = u.x; v[1] = u.y; }
+	static __device__ __forceinline__ void st(float *a, const float (&v)[2]) { *reinterpret_cast<float2 *>(a) = make_float2(v[0], v[1]); }
+};
+template <> struct ColsF<4> {
+	static __device__ __forceinline__ void ld(const float *a, float (&v)[4]) { const float4 u = *reinterpret_cast<const float4 *>(a); v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w; }
+	static __device__ __forceinline__ void ldg(const float *a, float (&v)[4]) { const float4 u = __ldg(reinterpret_cast<const float4 *>(a)); v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w; }
+	static __device__ __forceinline__ void st(float *a, const float (&v)[4]) { *reinterpret_cast<float4 *>(a) = make_float4(v[0], v[1], v[2], v[3]); }
+};
+
+template <int K8, int LPR, int WARPS, int CW>
+__global__ void __launch_bounds__(32 * WARPS)
+k_channelize_ovl_rdft(const uint8_t *__restrict__ in, size_t stream_stride, int hpad, const float *__restrict__ ptab,
+                      const float2 *__restrict__ tw, const unsigned *__restrict__ meta, float *__restrict__ dm, int nch, int ngrp,
+                      size_t nsamp)
+{
+	using P = RdftPlan<K8, LPR, WARPS>;
+	constexpr int K = P::K, N2 = P::N2, ROWS = P::ROWS, T = ROWS * WARPS, NU = K / CW;
+	constexpr int GF = P::GROUP / 4;                  /* ring row pitch in floats (a row plus 16 bytes, as the rdft tile) */
+	static_assert(T % 4 == 0 && K % 4 == 0, "rows go four at a time; columns in 16-byte units");
+	extern __shared__ __align__(16) unsigned char smem[];
+	const int l = threadIdx.x & 31;
+	const int w = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+	const int blk = blockIdx.x, s = blockIdx.y, g = blockIdx.z;
+	const int HR = (hpad + K - 1) / K, NR = HR + T, n0 = HR * K - hpad;
+	float *ring = reinterpret_cast<float *>(smem);
+	const float4 *stw = reinterpret_cast<const float4 *>(smem + (size_t)NR * P::GROUP);             /* [slot][n2] (Tr, Ti) */
+	unsigned long long *bar = reinterpret_cast<unsigned long long *>(smem + (size_t)NR * P::GROUP + P::TW_BYTES);
+	const uint8_t *src_s = in + (size_t)s * stream_stride;          /* sample 0 of the submit; the history sits in front */
+	const unsigned m = __shfl_sync(0xffffffffu, meta[(size_t)s * ngrp + g], 0);
+
+	if (threadIdx.x == 0) mbar_init(bar, 1);
+	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+	/* slots sorted by column as in k_channelize_rdft */
+	unsigned pw = 0, neg = 0;
+	int bnd0, bnd1;
+	{
+		int cnt[3] = { 0, 0, 0 };
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) {
+			const unsigned r = (m >> (2 * c)) & 3u;
+			const int cls = r == 0 ? 0 : r == 2 ? 1 : 2;
+#pragma unroll
+			for (int q = 0; q < 3; q++) cnt[q] += (cls == q);
+		}
+		bnd0 = cnt[0]; bnd1 = bnd0 + cnt[1];
+		int pos[3] = { 0, bnd0, bnd1 };
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) {
+			const unsigned r = (m >> (2 * c)) & 3u;
+			const int cls = r == 0 ? 0 : r == 2 ? 1 : 2;
+			int at = 0;
+#pragma unroll
+			for (int q = 0; q < 3; q++) { at = (cls == q) ? pos[q] : at; pos[q] += (cls == q); }
+			pw |= (unsigned)c << (3 * at);
+			neg |= (unsigned)(r == 3) << at;
+		}
+	}
+	{
+		const uint4 *tsrc = reinterpret_cast<const uint4 *>(tw + ((size_t)s * ngrp + g) * N2 * CH_GROUP);
+		uint4 *tdst = reinterpret_cast<uint4 *>(smem + (size_t)NR * P::GROUP);
+		constexpr int PER16 = N2 * 8 / 16;
+		for (int q = threadIdx.x; q < P::TW_BYTES / 16; q += 32 * WARPS) {
+			const int j = q / PER16, off = q - j * PER16;
+			cp_async16(tdst + q, tsrc + ((pw >> (3 * j)) & 7u) * PER16 + off);
+		}
+		cp_async_commit();
+		cp_async_wait_all();
+	}
+	__syncthreads();
+
+	const long long row_base = (long long)blk * OUTBLK;
+	const int rows_here = (int)min((size_t)OUTBLK, nsamp - (size_t)row_base);
+	const int nstep = (rows_here + T - 1) / T;
+	/* rows q (relative to the block) live in slot (q + HR) mod NR */
+	auto issue = [&](int i) {
+		if (elect_one()) {
+			const int q0 = i == 0 ? -HR : i * T, q1 = min((i + 1) * T, rows_here);
+			mbar_expect_tx(bar, (unsigned)(((q1 - q0) * K - (i == 0 ? n0 : 0)) * 4));
+			int sl = (q0 + HR) % NR;
+			for (int q = q0; q < q1; q++) {
+				const int s0 = q == -HR ? n0 : 0;
+				const long long smp = (row_base + q) * K + s0;           /* >= -hpad: before the submit means in the history */
+				bulk_g2s(ring + (size_t)sl * GF + s0, src_s + smp * 4, (unsigned)((K - s0) * 4), bar);
+				sl = sl + 1 == NR ? 0 : sl + 1;
+			}
+		}
+	};
+	if (w == 0) issue(0);
+	const int nc = min(CH_GROUP, nch - g * CH_GROUP);
+	const int row = l % ROWS, h = l / ROWS;
+	const int gp0 = h * P::PER, gp1 = min(K8, gp0 + P::PER);
+
+	for (int i = 0; i < nstep; i++) {
+		const int j0 = i * T, nrows = min(T, rows_here - j0);
+		mbar_wait(bar, (unsigned)(i & 1));
+
+		/* 2. the pre-sum of rows j0 .. j0 + nrows - 1 (a last partial group of four runs on stale slots and is not stored) */
+		for (int u = threadIdx.x; u < NU; u += 32 * WARPS) {
+			const int nn = u * CW;
+			const int rlo = -((nn + hpad) / K);            /* terms r = rlo .. 0, the same for the CW columns */
+			const float *pr = ptab + nn + hpad;             /* p of term r at pr + r*K */
+#pragma unroll 1
+			for (int jb = 0; jb < nrows; jb += 4) {
+				float acc[4][CW], pp[4][CW];
+#pragma unroll
+				for (int b = 0; b < 4; b++)
+#pragma unroll
+					for (int c = 0; c < CW; c++) acc[b][c] = pp[b][c] = 0.0f;
+				/* input row j0 + jb + t for t = rlo .. 3 feeds row j0 + jb + b as its term r = t - b; pp[(t - rlo) mod 4]
+				 * holds p of term t, which rows b = 0 .. 3 use at t .. t + 3 */
+				int sl = (j0 + jb + rlo + HR) % NR;
+#pragma unroll 1
+				for (int t0 = rlo; t0 <= 3; t0 += 4) {
+#pragma unroll
+					for (int k = 0; k < 4; k++) {
+						const int t = t0 + k;
+						if (t <= 3) {
+							float x[CW];
+							ColsF<CW>::ld(ring + (size_t)sl * GF + nn, x);
+							sl = sl + 1 == NR ? 0 : sl + 1;
+							if (t <= 0) ColsF<CW>::ldg(pr + t * K, pp[k]);
+#pragma unroll
+							for (int b = 0; b < 4; b++) {
+								if (t - b >= rlo && t - b <= 0) {
+#pragma unroll
+									for (int c = 0; c < CW; c++) acc[b][c] = __fmaf_rn(pp[(k - b) & 3][c], x[c], acc[b][c]);
+								}
+							}
+						}
+					}
+				}
+#pragma unroll
+				for (int b = 0; b < 4; b++) ColsF<CW>::st(ring + (size_t)((j0 + jb + b) % NR) * GF + nn, acc[b]);
+			}
+		}
+		__syncthreads();
+
+		/* 3. the DFT half, k_channelize_rdft's operations on the z row of step row w*ROWS + row */
+		const int j = w * ROWS + row;
+		const unsigned char *ra = reinterpret_cast<const unsigned char *>(ring + (size_t)((j0 + j) % NR) * GF);
+		float2 A[CH_GROUP], B[CH_GROUP];
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) A[c] = B[c] = make_float2(0.f, 0.f);
+
+#pragma unroll 1
+		for (int gp = gp0; gp < gp1; gp++) {              /* n2 = 2 gp, 2 gp + 1 */
+			const float2 x0 = *reinterpret_cast<const float2 *>(ra + 0 * P::K + gp * 8);
+			const float2 x1 = *reinterpret_cast<const float2 *>(ra + 1 * P::K + gp * 8);
+			const float2 x2 = *reinterpret_cast<const float2 *>(ra + 2 * P::K + gp * 8);
+			const float2 x3 = *reinterpret_cast<const float2 *>(ra + 3 * P::K + gp * 8);
+			const float2 s02 = fadd2_rn(x0, x2), s13 = fadd2_rn(x1, x3);
+			const float2 y0 = fadd2_rn(s02, s13), y2 = fsub2(s02, s13);
+			const float2 d02 = fsub2(x0, x2), d13 = fsub2(x1, x3);
+			const float4 *tj = stw + gp;
+#define ACB_ORD_E(J, Y)                                                                    \
+			{                                                                                      \
+				const float4 u = tj[(J) * (N2 / 2)];                                                   \
+				A[J] = ffma2(make_float2(Y.x, Y.x), make_float2(u.x, u.y), A[J]);                      \
+				A[J] = ffma2(make_float2(Y.y, Y.y), make_float2(u.z, u.w), A[J]);                      \
+			}
+#define ACB_ORD_O(J)                                                                       \
+			{                                                                                      \
+				const float4 u = tj[(J) * (N2 / 2)];                                                   \
+				A[J] = ffma2(make_float2(d02.x, d02.x), make_float2(u.x, u.y), A[J]);                  \
+				B[J] = ffma2(make_float2(d13.x, d13.x), make_float2(u.x, u.y), B[J]);                  \
+				A[J] = ffma2(make_float2(d02.y, d02.y), make_float2(u.z, u.w), A[J]);                  \
+				B[J] = ffma2(make_float2(d13.y, d13.y), make_float2(u.z, u.w), B[J]);                  \
+			}
+#define ACB_ORD_C0(J) if ((J) >= bnd0) goto o1_##J; ACB_ORD_E(J, y0)
+#define ACB_ORD_C1(J) o1_##J: if ((J) >= bnd1) goto o2_##J; ACB_ORD_E(J, y2)
+#define ACB_ORD_C2(J) o2_##J: ACB_ORD_O(J)
+#define ACB_ORD_COL(C) C(0) C(1) C(2) C(3) C(4) C(5) C(6) C(7)
+			ACB_ORD_COL(ACB_ORD_C0) goto omacs_done;
+			ACB_ORD_COL(ACB_ORD_C1) goto omacs_done;
+			ACB_ORD_COL(ACB_ORD_C2)
+			omacs_done:;
+#undef ACB_ORD_COL
+#undef ACB_ORD_C2
+#undef ACB_ORD_C1
+#undef ACB_ORD_C0
+#undef ACB_ORD_O
+#undef ACB_ORD_E
+		}
+		/* 4. every thread is done with the z rows: their slots take the next step's input (the async proxy writes where the
+		 * generic proxy wrote and read) */
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+		__syncthreads();
+		if (w == 0 && i + 1 < nstep) issue(i + 1);
+#pragma unroll
+		for (int step = ROWS; step < 32; step *= 2) {
+#pragma unroll
+			for (int jj = 0; jj < CH_GROUP; jj++) {
+				A[jj].x = __fadd_rn(A[jj].x, __shfl_xor_sync(0xffffffffu, A[jj].x, step));
+				A[jj].y = __fadd_rn(A[jj].y, __shfl_xor_sync(0xffffffffu, A[jj].y, step));
+				B[jj].x = __fadd_rn(B[jj].x, __shfl_xor_sync(0xffffffffu, B[jj].x, step));
+				B[jj].y = __fadd_rn(B[jj].y, __shfl_xor_sync(0xffffffffu, B[jj].y, step));
+			}
+		}
+		const size_t mrow = (size_t)row_base + j0 + j;
+		if (h == 0 && j < nrows) {
+			float *o = dm + ((size_t)s * nsamp + mrow) * nch + g * CH_GROUP;
+#pragma unroll
+			for (int jj = 0; jj < CH_GROUP; jj++) {
+				const float sg = ((neg >> jj) & 1u) ? -1.0f : 1.0f;
+				const float re = __fadd_rn(A[jj].x, __fmul_rn(sg, B[jj].y)), im = __fadd_rn(A[jj].y, -__fmul_rn(sg, B[jj].x));
+				const float e = envelope(make_float2(re, im));           /* in double: float input has no bound */
+				const int c = (int)((pw >> (3 * jj)) & 7u);
+				if (c < nc) o[c] = e;
+			}
+		}
+	}
+}
+
+/* shared memory of k_channelize_ovl_rdft: the (HR + T)-row ring, the twiddles and the barrier */
+template <int K8, int LPR, int WARPS>
+static int ovl_rdft_smem(int hpad)
+{
+	using P = RdftPlan<K8, LPR, WARPS>;
+	const int HR = (hpad + P::K - 1) / P::K;
+	return (HR + P::ROWS * WARPS) * P::GROUP + P::TW_BYTES + 8;
+}
+
+template <int K8, int LPR, int WARPS, int CW>
+static int launch_ovl_rdft_t(const uint8_t *in, size_t stream_stride, int hpad, const float *p, const float2 *tw,
+                             const unsigned *meta, float *dm, int nch, int nstreams, int nblk, size_t nsamp, cudaStream_t stream)
+{
+	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
+	const int smem = ovl_rdft_smem<K8, LPR, WARPS>(hpad);
+	auto kern = k_channelize_ovl_rdft<K8, LPR, WARPS, CW>;
+	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	if (e != cudaSuccess) return (int)e;
+	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	if (e != cudaSuccess) return (int)e;
+	dim3 grid(nblk, nstreams, ngrp);
+	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, hpad, p, tw, meta, dm, nch, ngrp, nsamp);
+	return (int)cudaGetLastError();
+}
+
+/* float32 real input, taps > K (hpad > 0), K in the rdft's five rates, every channel on the 12.5 kHz raster; `in` = sample 0
+ * of stream 0's submit with each stream's hpad-sample history right in front of it (d_real); `nsamp` output rows per
+ * stream, any count; `p` = taps_pad floats, fl(K*h) behind hpad - H zeros */
+int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
+                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	if (nsamp == 0) return 0;
+	if (hpad <= 0 || hpad % 4) return (int)cudaErrorInvalidValue;           /* 16-byte copies; taps <= K has no history */
+	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
+	const float2 *t4 = reinterpret_cast<const float2 *>(tw);
+	const int nblk = (int)((nsamp + OUTBLK - 1) / OUTBLK);
+	/* 4 warps; T = 64 rows per step at K = 200 / 240, 32 at 400 / 480, 16 at 800.  Columns per pre-sum thread: 2 where K/4
+	 * units would leave most of the 128 threads idle */
+#define ACB_ORD_GO(K8, LPR, CW) launch_ovl_rdft_t<K8, LPR, 4, CW>(i8, stream_stride, hpad, p, t4, meta, dm, nch, nstreams, nblk, nsamp, stream)
+	if (K == 200) return ACB_ORD_GO(25, 2, 2);
+	if (K == 240) return ACB_ORD_GO(30, 2, 2);
+	if (K == 400) return ACB_ORD_GO(50, 4, 4);
+	if (K == 480) return ACB_ORD_GO(60, 4, 4);
+	if (K == 800) return ACB_ORD_GO(100, 8, 4);
+#undef ACB_ORD_GO
+	return (int)cudaErrorInvalidValue;
+}
+
 bool channelize_dft_supports(int K) { return K == 160 || K == 192; }
 
 /* u8 IQ, K in {160, 192} (the reference's two rates), taps == K, every channel on the 12.5 kHz raster

@@ -63,7 +63,8 @@ typedef struct {
 	                           group delay of about (taps - K)/(2K) output samples is not compensated.  The context
 	                           keeps each stream's last H samples (rounded up to 16 bytes) across submits; acb_reset
 	                           clears them.  ACB_FLAG_FAST_CHANNELIZER is accepted and the exact kernel runs;
-                           ACB_FLAG_FAST_FILTER selects the polyphase fast form of this filter. */
+                           ACB_FLAG_FAST_FILTER (u8, CS16) and ACB_FLAG_FAST_FILTER_REAL (real input) select
+                           the polyphase fast form of this filter. */
 } acb_config_t;
 
 #define ACB_MAXTAPS_PER_K 16          /* longest overlapping window, in decimation periods */
@@ -94,7 +95,22 @@ typedef struct {
                                          within 1e-5*S of the exact form's and within 1e-6*S of the float64 definition;
                                          decoded messages are the same.  Anything else (a stream off the raster, a table given
                                          through acb_set_wf, another K, real input) runs the exact kernel, as does taps <= K,
-                                         where this flag has no effect. */
+                                         where this flag has no effect.  Real input has its own bit,
+                                         ACB_FLAG_FAST_FILTER_REAL. */
+#define ACB_FLAG_FAST_FILTER_REAL 32   /* taps > K on real-input contexts (ACB_FLAG_REAL_INPUT) with K = 200, 240, 400, 480 or
+                                         800, every stream planned by acb_set_plan_air with every channel on the 12.5 kHz
+                                         raster (acb_fast_plan_air returns 1): the polyphase fast form for real input.  The
+                                         window is pre-summed into one K-sample real row per output,
+                                           z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K],  p = fl(K * h)  (h: acb_build_lowpass)
+                                         (ascending tap order, one FMA per term, terms before the stream start omitted), and
+                                         each channel's bin of that row is taken exactly as ACB_FLAG_FAST_CHANNELIZER takes it
+                                         from a row of input (k_channelize_rdft's operations, |D| in double): taps/K + ~10
+                                         FP32 lane-ops per sample for 8 channels instead of 4*C*taps/K.  NOT the exact form's
+                                         operation order: per output row, with S = sum |x|*|w|, the envelope is within 1e-5*S
+                                         of the exact form's and within 1e-6*S of the float64 definition; decoded messages are
+                                         the same.  Anything else (acb_set_wf tables, a stream off the raster, another K) runs
+                                         the exact kernel, unchanged, as does taps <= K; on u8 and CS16 contexts this flag has
+                                         no effect, and ACB_FLAG_FAST_FILTER alone selects nothing on a real context. */
 #define ACB_FLAG_REAL_INPUT 2         /* Airspy front-end (air.c): float32 REAL samples at IF = rate/4,
                                          rate = K*12500; use acb_set_plan_air / acb_submit_real_host */
 
@@ -335,7 +351,7 @@ typedef struct {
 	double   demod_ms;          /* accumulated device time from a demod kernel's start to the end of its block FEC */
 	uint64_t chan_launches, demod_launches;
 	uint64_t fast_chan_launches; /* channelizer launches that took a fast form: ACB_FLAG_FAST_CHANNELIZER's (taps = K) or
-	                                ACB_FLAG_FAST_FILTER's (taps > K) */
+	                                ACB_FLAG_FAST_FILTER's or ACB_FLAG_FAST_FILTER_REAL's (taps > K) */
 	uint64_t frames_lost;       /* frames that found the device ring full (ACB_ERR_OVERFLOW was returned once per submit) */
 	double   host_ms;           /* accumulated wall time the consumer thread spent ordering and queuing frames */
 } acb_stats_t;
