@@ -17,6 +17,7 @@ LIB_PATH = PKG / "libacars_b200.so"
 
 OUTBLK = 1024
 TXTMAX = 250
+FLAG_FAST_WIDEBAND = 64          # ACB_FLAG_FAST_WIDEBAND: the fast forms for any K % 8 == 0 and any channel count
 
 
 class Config(C.Structure):

@@ -55,7 +55,19 @@ struct RingCtl {
 constexpr int CH_TILE = 128;          /* threads per channelizer CTA (2 output rows each) */
 constexpr int CH_GROUP = 8;           /* channels accumulated per pass */
 
+/* wideband fast form (k_channelize_wb): channels per CTA, channel slots per thread, slot capacity per channel tile (every
+ * residue class padded to whole groups of WB_CB), the per-(stream, tile) plan in ints: groups, E table, (k, channel) per slot */
+constexpr int WB_THREADS = 288;
+constexpr int WB_CTILE = 256;
+constexpr int WB_CB = 4;
+constexpr int WB_SLOTS = WB_CTILE + 4 * (WB_CB - 1) + 4;
+constexpr int WB_META = 2 + 2 * WB_SLOTS;
+
 } // namespace acb
+
+/* hostmath.cpp: the wideband form's twiddle table E[r + K - 1], r in (-K, K), with the fast planners' expression for the
+ * exponent r = (k*n2) % K; variant -1: u8 (acb_fast_plan), else a CS16 variant (acb_fast_plan_cs16).  1 on success. */
+extern "C" int acb_wb_twiddles(int variant, int K, float *E);
 
 /* kernels.cu entry points (host-callable launchers) */
 struct CUstream_st;
@@ -87,6 +99,8 @@ int launch_channelize_dft_cs16(const void *in, size_t stream_stride, const float
                                int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
                                const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
+int launch_channelize_wb(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *E,
+                         const int *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 bool channelize_rdft_supports(int K);
 int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
                            int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);

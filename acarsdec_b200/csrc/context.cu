@@ -92,7 +92,11 @@ struct acb_ctx {
 	bool fast_ovl;               /* taps > K and the polyphase form: ACB_FLAG_FAST_FILTER on u8 / CS16 with a K
 	                                k_channelize_ovl_fast takes, ACB_FLAG_FAST_FILTER_REAL on real input with a K
 	                                k_channelize_ovl_rdft takes */
-	float *d_p;                  /* fast_ovl: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
+	bool wb;                     /* ACB_FLAG_FAST_WIDEBAND on u8 / CS16, K % 8 == 0, taps >= K, and neither of the
+	                                above selects a narrow kernel: k_channelize_wb */
+	float *d_wbE;                /* wb: the twiddle table(s) E of acb_wb_twiddles, 2K - 1 (Tr, Ti) each; CS16: one per variant */
+	int *d_wbmeta;               /* wb: [stream][channel tile][WB_META] residue-sorted slots (upload_wb_plan) */
+	float *d_p;                  /* fast_ovl, wb at taps > K: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
 	bool fold8;                  /* fast form: fold the row in half first (8-way split, K/8 MACs per channel) */
 	int demod_lanes;             /* lanes per channel in k_demod: 8 for small contexts, else 4 */
 	float *d_tw;                 /* fast form: [stream][grp][8 ch][K/4] (Tr, Ti) twiddles */
@@ -350,6 +354,10 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->fast_ovl = c->taps > cfg->K &&
 	              (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_FILTER_REAL) && channelize_rdft_supports(cfg->K)
 	                                             : (cfg->flags & ACB_FLAG_FAST_FILTER) && channelize_dft_supports(cfg->K));
+	c->wb = (cfg->flags & ACB_FLAG_FAST_WIDEBAND) && c->in_kind != IN_KIND_F32REAL && cfg->K % 8 == 0 && c->taps >= cfg->K &&
+	        !c->fast && !c->fast_ovl;
+	c->d_wbE = nullptr;
+	c->d_wbmeta = nullptr;
 	c->d_p = nullptr;
 	c->fast_ok.assign(cfg->nstreams, 0);
 	c->fold8 = true;             /* K/8 instead of K/4 MACs per channel than the plain 4-way split */
@@ -370,7 +378,18 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaMalloc(&c->d_tw, (size_t)cfg->nstreams * c->ngrp * CH_GROUP * (cfg->K / 4) * 2 * sizeof(float)));
 		CU(cudaMalloc(&c->d_twmeta, (size_t)cfg->nstreams * c->ngrp * sizeof(unsigned)));
 	}
-	if (c->fast_ovl) {
+	if (c->wb) {
+		const int ntab = c->in_kind == IN_KIND_CS16IQ ? 2 : 1;
+		const size_t per = (size_t)(2 * cfg->K - 1) * 2;
+		std::vector<float> E(ntab * per);
+		for (int t = 0; t < ntab; t++)
+			acb_wb_twiddles(c->in_kind == IN_KIND_CS16IQ ? t : -1, cfg->K, &E[t * per]);
+		CU(cudaMalloc(&c->d_wbE, E.size() * sizeof(float)));
+		if (int r = upload(c, c->d_wbE, E.data(), E.size() * sizeof(float))) return r;
+		const size_t nct = (size_t)(cfg->nch + WB_CTILE - 1) / WB_CTILE;
+		CU(cudaMalloc(&c->d_wbmeta, (size_t)cfg->nstreams * nct * WB_META * sizeof(int)));
+	}
+	if (c->fast_ovl || (c->wb && c->hpad)) {
 		/* the polyphase weights p[i] = fl(K * h[i]), laid out like the exact table (taps_pad entries, the hpad - H in front
 		 * zero): the same for every channel and stream; with the twiddles' 1/K the pre-sum's bin carries h[i] * scale */
 		std::vector<float> h(c->taps), p(c->taps_pad, 0.0f);
@@ -447,6 +466,7 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 		cudaFree(c->d_hist);
 		cudaFree(c->d_wf4); cudaFree(c->d_state);
 		cudaFree(c->d_tw); cudaFree(c->d_twmeta); cudaFree(c->d_p);
+		cudaFree(c->d_wbE); cudaFree(c->d_wbmeta);
 		for (int i = 0; i < NPIPE; i++) {
 			cudaFree(c->d_dm[i]); cudaEventDestroy(c->ev_k1_done[i]); cudaEventDestroy(c->ev_dm_free[i]);
 			cudaEventDestroy(c->ev_k2_done[i]); cudaEventDestroy(c->ev_ring_read[i]);
@@ -516,6 +536,37 @@ static int upload_fast_plan(acb_ctx *c, int stream, bool ok, const std::vector<i
 	return ACB_OK;
 }
 
+/* wideband form: per channel tile, the channel slots sorted by bin residue (k/2) mod 4 and each residue class padded to
+ * whole groups of WB_CB (channel -1), so that every thread of k_channelize_wb multiplies one Y' row; `etab` selects the
+ * twiddle table (CS16: the variant).  `ok` false leaves the stream on the exact kernel. */
+static int upload_wb_plan(acb_ctx *c, int stream, bool ok, const std::vector<int> &kbin, int etab)
+{
+	if (!ok) return ACB_OK;
+	const int nch = c->cfg.nch, nct = (nch + WB_CTILE - 1) / WB_CTILE;
+	std::vector<int> meta((size_t)nct * WB_META, 0);
+	for (int z = 0; z < nct; z++) {
+		int *m = &meta[(size_t)z * WB_META];
+		int slot = 0;
+		for (int res = 0; res < 4; res++) {
+			for (int ch = z * WB_CTILE; ch < std::min(nch, (z + 1) * WB_CTILE); ch++) {
+				if ((((kbin[ch] / 2) % 4) + 4) % 4 != res) continue;
+				m[2 + 2 * slot] = kbin[ch];
+				m[3 + 2 * slot] = ch;
+				slot++;
+			}
+			for (; slot % WB_CB; slot++) {
+				m[2 + 2 * slot] = 0;
+				m[3 + 2 * slot] = -1;
+			}
+		}
+		m[0] = slot / WB_CB;
+		m[1] = etab;
+	}
+	if (int r = upload(c, c->d_wbmeta + (size_t)stream * meta.size(), meta.data(), meta.size() * sizeof(int))) return r;
+	c->fast_ok[stream] = 1;
+	return ACB_OK;
+}
+
 extern "C" int acb_set_plan(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
@@ -539,11 +590,12 @@ extern "C" int acb_set_plan_at(acb_ctx_t *c, int stream, const unsigned *freqs_h
 		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
 	}
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
+	const int K = c->cfg.K, N2 = K / 4;
+	std::vector<int> kbin(nch);
+	if (c->wb) return upload_wb_plan(c, stream, acb_fast_plan(freqs_hz, nch, K, fc, kbin.data(), nullptr) == 1, kbin, 0);
 	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	/* Fast forms (taps = K, or the overlapping window's polyphase form): per-channel bin numbers and twiddles, when every
 	 * channel sits on the raster */
-	const int K = c->cfg.K, N2 = K / 4;
-	std::vector<int> kbin(nch);
 	std::vector<float> tw1((size_t)nch * N2 * 2);
 	const bool ok = acb_fast_plan(freqs_hz, nch, K, fc, kbin.data(), tw1.data()) == 1;
 	return upload_fast_plan(c, stream, ok, kbin, tw1);
@@ -780,7 +832,7 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		/* whole 1024-row blocks through the pipeline kernel, the remaining rows (submits of 4-byte
 		 * samples may carry any count) and unaligned K through the generic one */
 		const int fast = c->use_generic ? 0 : nsamp / OUTBLK;
-		bool dft = c->fast || c->fast_ovl;           /* every stream planned on the raster? */
+		bool dft = c->fast || c->fast_ovl || c->wb;  /* every stream planned on the raster? */
 		for (int s = 0; dft && s < c->cfg.nstreams; s++) dft = c->fast_ok[s] != 0;
 		bool all_rows = false;                       /* the fast CS16 kernel takes partial blocks too */
 		bool ovl_fast = false;                       /* the polyphase form ran: it omits the terms before the stream start itself */
@@ -794,7 +846,16 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			hist.base = d_iq - (size_t)c->hpad * 4;
 			hist.stride = stride;
 		}
-		if (dft && c->fast_ovl && c->in_kind == IN_KIND_F32REAL) {
+		if (dft && c->wb) {
+			/* every row of the submit, CS16 partial blocks included; at taps > K the terms before the stream start are
+			 * omitted in the kernel */
+			r = launch_channelize_wb(c->in_kind, d_iq, stride, hist, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                         c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			c->stats.kernel_launches++;
+			c->stats.fast_chan_launches++;
+			all_rows = true;
+			ovl_fast = true;
+		} else if (dft && c->fast_ovl && c->in_kind == IN_KIND_F32REAL) {
 			/* the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
 			r = launch_channelize_ovl_rdft(d_iq, stride, c->hpad, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
 			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
@@ -1077,8 +1138,10 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<int> kbin(nch);
+	if (c->wb)
+		return upload_wb_plan(c, stream, acb_fast_plan_cs16(variant, freqs_hz, nch, c->cfg.K, fc, kbin.data(), nullptr) == 1, kbin, variant);
+	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
 	const bool ok = acb_fast_plan_cs16(variant, freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;
 	return upload_fast_plan(c, stream, ok, kbin, tw1);

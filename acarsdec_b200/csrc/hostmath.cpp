@@ -25,6 +25,7 @@
 
 #include "../../include/acars_b200.h"
 #include "frame_sm.h"
+#include "acb_internal.h"
 
 /* cos/sin(k*pi/32), k < 64, as double-double (hi, lo) pairs for the demod kernel's VCO sincos
  * (demod_core.h sincos_vco); long double (64-bit mantissa) is ample for the non-zero entries, the
@@ -303,6 +304,28 @@ extern "C" int acb_fast_plan_cs16(int variant, const unsigned *freqs_hz, int nch
 			const double ph = -2.0 * M_PI * (double)(((long long)k * n2) % K) / (double)K;
 			tw[((size_t)ch * N2 + n2) * 2] = (float)(cos(ph) / K * scale);
 			tw[((size_t)ch * N2 + n2) * 2 + 1] = (float)(sin(ph) / K * scale);
+		}
+	}
+	return 1;
+}
+
+extern "C" int acb_wb_twiddles(int variant, int K, float *E)
+{
+	/* Every twiddle the two planners above write depends on k and n2 only through r = (k*n2) % K (C remainder: the sign of
+	 * k), so one table indexed by r in (-K, K) serves every channel of a context (k_channelize_wb).  Both signs are kept:
+	 * cos(2*pi*(r + K)/K) need not round like cos(2*pi*r/K).  The expressions are the planners' own, token for token. */
+	if (!E || K <= 0 || K > ACB_MAXK || (K & 3)) return 0;
+	if (variant != -1 && variant != ACB_CS16_SOAPY && variant != ACB_CS16_SDRPLAY) return 0;
+	const double scale = variant == ACB_CS16_SOAPY ? 1.0 / 32768.0 : 0.25;
+	for (int r = -(K - 1); r < K; r++) {
+		const double ph = -2.0 * M_PI * (double)r / (double)K;
+		float *o = E + (size_t)(r + K - 1) * 2;
+		if (variant == -1) {
+			o[0] = (float)(cos(ph) / K / 127.5);
+			o[1] = (float)(sin(ph) / K / 127.5);
+		} else {
+			o[0] = (float)(cos(ph) / K * scale);
+			o[1] = (float)(sin(ph) / K * scale);
 		}
 	}
 	return 1;

@@ -1287,6 +1287,242 @@ int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, c
 }
 
 /* ------------------------------------------------------------------------------------------
+ * K1, wideband fast form (ACB_FLAG_FAST_WIDEBAND; DESIGN.md §4): the boxcar fast form (taps = K, orc_channelize_dft8*) and
+ * the polyphase form (taps > K, orc_channelize_ovl_fast*) for any K % 8 == 0 up to ACB_MAXK and any channel count.  The
+ * narrow kernels above put one group of 8 channels in a CTA and redo the row's shared work for every group; here one CTA
+ * takes rows_per_cta rows (tiles of T = 4*RB) of one stream and up to WB_CTILE channels:
+ *
+ *   front half (once per row for all channels): the integer fold and 4-point split of the row (boxcar), or the pre-sum
+ *     z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K] in ascending tap order followed by the float fold and split
+ *     (polyphase), into Y'[residue][row][n2] in shared memory.  Samples and weights are read through L1/L2 with the
+ *     columns n2 owned by consecutive threads; every fetch lies in [-hpad, nsamp*K) samples of the stream, the samples
+ *     before the submit coming from the history (u8: the context's buffer; CS16: in front of the rows), and terms
+ *     whose row lies before the stream start are omitted (as k_channelize_ovl_fast; for u8 the zero bytes of a cleared
+ *     history would convert to -127.37, not to 0).
+ *   back half (one SIMT complex GEMM per residue class): a thread owns RB rows x WB_CB channel slots of one residue and
+ *     walks n2 upwards with the restatements' four fmaf chains per output.  The twiddles come from ONE table E of
+ *     2K - 1 entries in shared memory, E[r] = the planner's T for (k*n2) % K = r (hostmath.cpp: acb_wb_twiddles): a
+ *     channel's index moves by k modulo K in C-remainder form, so T_c[n2] = E[(k_c*n2) % K] bit for bit.  The slots are
+ *     sorted by residue and padded per residue to whole groups of WB_CB (context.cu: upload_wb_plan), so a thread's Y'
+ *     loads are one address for the whole group and mostly for the whole warp.
+ *
+ * meta per (stream, channel tile): [0] groups of WB_CB slots, [1] which E table (CS16: the variant), then (k, channel)
+ * per slot, channel -1 for padding.
+ * ---------------------------------------------------------------------------------------- */
+template <int KIND, bool OVL, int RB>
+__global__ void __launch_bounds__(WB_THREADS, 2)
+k_channelize_wb(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ hist, size_t hist_stride,
+                int hpad, unsigned long long pos0, const float *__restrict__ pw, const float2 *__restrict__ E,
+                const int *__restrict__ meta, float *__restrict__ dm, int K, int nch, int nctile, size_t nsamp, int rows_per_cta)
+{
+	constexpr int T = 4 * RB, BPS = KIND == IN_CS16IQ ? 4 : 2;
+	const int N8 = K >> 3;
+	extern __shared__ __align__(16) unsigned char smem[];
+	float2 *Ys = reinterpret_cast<float2 *>(smem);                 /* [residue][row][n2] */
+	float2 *Es = Ys + (size_t)4 * T * N8;                           /* E[r], r in (-K, K), at Es[r + K - 1] */
+	const int s = blockIdx.y;
+	const int *ms = meta + ((size_t)s * nctile + blockIdx.z) * WB_META;
+	const int ng = ms[0];
+	const float2 *Eg = E + (size_t)ms[1] * (2 * K - 1);
+	for (int i = threadIdx.x; i < 2 * K - 1; i += WB_THREADS) Es[i] = Eg[i];
+
+	/* back-half work item: row group rg (rows rg*RB ..), channel group cg */
+	const int rg = (int)threadIdx.x / ng, cg = (int)threadIdx.x - rg * ng;
+	int kk[WB_CB];                                /* the slots' channels are read again at the store: fewer live registers */
+#pragma unroll
+	for (int c = 0; c < WB_CB; c++) kk[c] = rg < 4 ? ms[2 + 2 * (cg * WB_CB + c)] : 0;
+	const int res = (((kk[0] / 2) % 4) + 4) % 4;                      /* slot 0 of a group is always a channel */
+
+	/* the CTA's rows in tiles of T; the bounds and stream pointers are recomputed from the parameters where they are used
+	 * rather than held across the back half, whose accumulators need the registers */
+	for (int t0 = 0; t0 < rows_per_cta; t0 += T) {
+		const size_t r0 = (size_t)blockIdx.x * rows_per_cta + t0;
+		if (r0 >= nsamp) break;
+		__syncthreads();                          /* E staged / the previous tile's Y' consumed */
+		const uint8_t *src_s = in + (size_t)s * stream_stride;
+		const uint8_t *hist_s = OVL ? hist + (size_t)s * hist_stride + (size_t)hpad * BPS : nullptr;   /* where sample 0 of the submit would sit */
+		for (int it = threadIdx.x; it < T * N8; it += WB_THREADS) {
+			const int j = it / N8, n2 = it - j * N8;
+			const size_t row = r0 + j;
+			float2 y[4] = { make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f) };
+			if (row < nsamp) {
+				if (!OVL) {
+					/* boxcar: the fold and split in integers, exact (orc_channelize_dft8*) */
+					const uint8_t *rp = src_s + row * (size_t)K * BPS;
+					int zi[4], zq[4];
+#pragma unroll
+					for (int n1 = 0; n1 < 4; n1++) {
+						const int ia = N8 * n1 + n2, ib = N8 * (n1 + 4) + n2;
+						if (KIND == IN_CS16IQ) {
+							const unsigned a = __ldg(reinterpret_cast<const unsigned *>(rp) + ia);
+							const unsigned b = __ldg(reinterpret_cast<const unsigned *>(rp) + ib);
+							zi[n1] = (int)(short)(a & 0xffffu) + (int)(short)(b & 0xffffu);
+							zq[n1] = (int)(short)(a >> 16) + (int)(short)(b >> 16);
+						} else {
+							const unsigned a = __ldg(reinterpret_cast<const unsigned short *>(rp) + ia);
+							const unsigned b = __ldg(reinterpret_cast<const unsigned short *>(rp) + ib);
+							zi[n1] = (int)(a & 0xffu) + (int)(b & 0xffu);
+							zq[n1] = (int)(a >> 8) + (int)(b >> 8);
+						}
+					}
+					const int bias = KIND == IN_CS16IQ ? 0 : 1020;
+					y[0] = make_float2((float)(zi[0] + zi[1] + zi[2] + zi[3] - bias), (float)(zq[0] + zq[1] + zq[2] + zq[3] - bias));
+					y[2] = make_float2((float)(zi[0] - zi[1] + zi[2] - zi[3]), (float)(zq[0] - zq[1] + zq[2] - zq[3]));
+					y[1] = make_float2((float)((zi[0] - zi[2]) + (zq[1] - zq[3])), (float)((zq[0] - zq[2]) - (zi[1] - zi[3])));
+					y[3] = make_float2((float)((zi[0] - zi[2]) - (zq[1] - zq[3])), (float)((zq[0] - zq[2]) + (zi[1] - zi[3])));
+				} else {
+					/* polyphase: the pre-sum of the eight samples n2 + e*K/8, then fold and split (orc_channelize_ovl_fast*) */
+					const unsigned long long mabs = pos0 + row;          /* row counted from the stream start */
+					float2 zz[8];
+#pragma unroll
+					for (int e = 0; e < 8; e++) {
+						const int nn = e * N8 + n2;
+						int rlo = -((nn + hpad) / K);
+						if ((unsigned long long)(-rlo) > mabs) rlo = -(int)mabs;   /* rows before the stream start: omitted */
+						const float *pr = pw + nn + hpad;
+						const long long smp0 = (long long)row * K + nn;
+						float a = 0.f, b = 0.f;
+						for (int r = rlo; r <= 0; r++) {
+							const long long smp = smp0 + (long long)r * K;   /* >= -hpad */
+							const uint8_t *q = smp < 0 ? hist_s + smp * BPS : src_s + smp * BPS;
+							float xr, xi;
+							if (KIND == IN_CS16IQ) {
+								const unsigned u = __ldg(reinterpret_cast<const unsigned *>(q));
+								xr = (float)(short)(u & 0xffffu);
+								xi = (float)(short)(u >> 16);
+							} else {
+								const unsigned u = __ldg(reinterpret_cast<const unsigned short *>(q));
+								xr = __fadd_rn((float)(u & 0xffu), -127.37f);
+								xi = __fadd_rn((float)(u >> 8), -127.37f);
+							}
+							const float pk = __ldg(pr + r * K);
+							a = __fmaf_rn(pk, xr, a);
+							b = __fmaf_rn(pk, xi, b);
+						}
+						zz[e] = make_float2(a, b);
+					}
+					float2 z[4];
+#pragma unroll
+					for (int n1 = 0; n1 < 4; n1++) z[n1] = fadd2_rn(zz[n1], zz[n1 + 4]);
+					const float2 s02 = fadd2_rn(z[0], z[2]), s13 = fadd2_rn(z[1], z[3]);
+					const float2 d02 = fsub2(z[0], z[2]);
+					const float2 wj = make_float2(__fadd_rn(z[1].y, -z[3].y), __fadd_rn(z[3].x, -z[1].x));   /* -j (z1 - z3) */
+					y[0] = fadd2_rn(s02, s13);
+					y[2] = fsub2(s02, s13);
+					y[1] = fadd2_rn(d02, wj);
+					y[3] = fsub2(d02, wj);
+				}
+			}
+#pragma unroll
+			for (int q = 0; q < 4; q++) Ys[((size_t)q * T + j) * N8 + n2] = y[q];
+		}
+		__syncthreads();
+		if (rg >= 4) continue;
+
+		float acc[RB][WB_CB][4];                  /* ax, ay, bx, by: re = ax - by, im = ay + bx */
+#pragma unroll
+		for (int j = 0; j < RB; j++)
+#pragma unroll
+			for (int c = 0; c < WB_CB; c++) acc[j][c][0] = acc[j][c][1] = acc[j][c][2] = acc[j][c][3] = 0.f;
+		int idx[WB_CB];
+#pragma unroll
+		for (int c = 0; c < WB_CB; c++) idx[c] = 0;
+		const float2 *Yr = Ys + ((size_t)res * T + rg * RB) * N8;
+		const float2 *Ec = Es + (K - 1);
+#pragma unroll 1
+		for (int n2 = 0; n2 < N8; n2++) {
+			float2 t[WB_CB];
+#pragma unroll
+			for (int c = 0; c < WB_CB; c++) {
+				t[c] = Ec[idx[c]];
+				int v = idx[c] + kk[c];           /* (k*(n2+1)) % K from (k*n2) % K, |k| < K/2 */
+				v = v >= K ? v - K : v;
+				idx[c] = v <= -K ? v + K : v;
+			}
+#pragma unroll
+			for (int j = 0; j < RB; j++) {
+				const float2 yv = Yr[j * N8 + n2];
+#pragma unroll
+				for (int c = 0; c < WB_CB; c++) {
+					acc[j][c][0] = __fmaf_rn(yv.x, t[c].x, acc[j][c][0]);
+					acc[j][c][1] = __fmaf_rn(yv.x, t[c].y, acc[j][c][1]);
+					acc[j][c][2] = __fmaf_rn(yv.y, t[c].x, acc[j][c][2]);
+					acc[j][c][3] = __fmaf_rn(yv.y, t[c].y, acc[j][c][3]);
+				}
+			}
+		}
+#pragma unroll
+		for (int j = 0; j < RB; j++) {
+			const size_t row = r0 + rg * RB + j;
+			if (row >= nsamp) continue;
+			float *o = dm + ((size_t)s * nsamp + row) * nch;
+#pragma unroll
+			for (int c = 0; c < WB_CB; c++) {
+				const int chc = __ldg(meta + ((size_t)s * nctile + blockIdx.z) * WB_META + 3 + 2 * (cg * WB_CB + c));
+				if (chc < 0) continue;
+				const float re = __fadd_rn(acc[j][c][0], -acc[j][c][3]), im = __fadd_rn(acc[j][c][1], acc[j][c][2]);
+				/* |D| in float, bounded as in k_channelize_dft1 / k_channelize_ovl_fast */
+				o[chc] = __fsqrt_rn(__fmaf_rn(re, re, __fmul_rn(im, im)));
+			}
+		}
+	}
+}
+
+/* rows per tile: 12 where two CTAs per SM still fit, Y' (4*K bytes per row) + E ((2K - 1) * 8 bytes) <= 113 KB (K <= 1808),
+ * else 8.  16-row tiles (RB = 4) would not fit their 64 accumulators in the 96 registers two 288-thread CTAs leave. */
+static int wb_rb(int K)
+{
+	return 16 * 3 * K + (2 * K - 1) * 8 <= 113 * 1024 ? 3 : 2;
+}
+
+template <int KIND, bool OVL, int RB>
+static int launch_wb_t(const uint8_t *in, size_t stream_stride, const Hist &h, const float *p, const float2 *E, const int *meta,
+                       float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	constexpr int T = 4 * RB;
+	const int smem = 4 * T * (K / 8) * 8 + (2 * K - 1) * 8;
+	const int nctile = (nch + WB_CTILE - 1) / WB_CTILE;
+	auto kern = k_channelize_wb<KIND, OVL, RB>;
+	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	if (e != cudaSuccess) return (int)e;
+	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	if (e != cudaSuccess) return (int)e;
+	/* tiles per CTA: up to 8 (E is staged once per CTA), fewer where that would leave less than four waves of two CTAs
+	 * per SM — a CTA runs its tiles in series, so a grid short of the SMs leaves them idle */
+	int dev = 0, nsm = 132;
+	if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+	const size_t tiles = (nsamp + T - 1) / T * (size_t)nstreams * nctile;
+	const int tpc = (int)std::max<size_t>(1, std::min<size_t>(8, tiles / ((size_t)8 * nsm)));
+	const int rows_per_cta = tpc * T;
+	dim3 grid((unsigned)((nsamp + rows_per_cta - 1) / rows_per_cta), nstreams, nctile);
+	kern<<<grid, WB_THREADS, smem, stream>>>(in, stream_stride, reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad, h.pos0,
+	                                         p, E, meta, dm, K, nch, nctile, nsamp, rows_per_cta);
+	return (int)cudaGetLastError();
+}
+
+/* u8 IQ or CS16 IQ, K % 8 == 0, K <= ACB_MAXK, any nch, every channel on the 12.5 kHz raster; taps = K (h.hpad = 0) or
+ * taps > K (`p` = taps_pad floats, fl(K*h) behind hpad - H zeros); `nsamp` output rows per stream, any count */
+int launch_channelize_wb(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *E,
+                         const int *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	if (nsamp == 0) return 0;
+	if ((K & 7) || K > 2048 || (mode != IN_U8IQ && mode != IN_CS16IQ)) return (int)cudaErrorInvalidValue;
+	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
+	const float2 *E2 = reinterpret_cast<const float2 *>(E);
+	const int rb = wb_rb(K);
+#define ACB_WB_GO(M, O, R) launch_wb_t<M, O, R>(i8, stream_stride, h, p, E2, meta, dm, K, nch, nstreams, nsamp, stream)
+#define ACB_WB_RB(M, O) return rb == 3 ? ACB_WB_GO(M, O, 3) : ACB_WB_GO(M, O, 2)
+	if (mode == IN_CS16IQ) {
+		if (h.hpad) ACB_WB_RB(IN_CS16IQ, true);
+		ACB_WB_RB(IN_CS16IQ, false);
+	}
+	if (h.hpad) ACB_WB_RB(IN_U8IQ, true);
+	ACB_WB_RB(IN_U8IQ, false);
+#undef ACB_WB_RB
+#undef ACB_WB_GO
+}
+
+/* ------------------------------------------------------------------------------------------
  * Fast form of the REAL-input channelizer (air.c:291-341 with the table of air.c:278-285): wf[i] = exp(-j*2*pi*k*i/K)/K is
  * a sampled exponential with k = (Fc - Fr + rate/4) / 12.5 kHz a whole number whenever the channels and the tuner
  * centre sit on the 12.5 kHz raster (air.c:66 puts Fc there), so D is bin k of the K-point DFT of a REAL row:

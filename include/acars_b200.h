@@ -111,6 +111,19 @@ typedef struct {
                                          the same.  Anything else (acb_set_wf tables, a stream off the raster, another K) runs
                                          the exact kernel, unchanged, as does taps <= K; on u8 and CS16 contexts this flag has
                                          no effect, and ACB_FLAG_FAST_FILTER alone selects nothing on a real context. */
+#define ACB_FLAG_FAST_WIDEBAND 64      /* u8 IQ and CS16 contexts (interleaved and planar) with K % 8 == 0 (K <= ACB_MAXK), any
+                                         nch, taps >= K, every stream planned by acb_set_plan, acb_set_plan_at,
+                                         acb_multi_set_plan or acb_set_plan_cs16 with acb_fast_plan / acb_fast_plan_cs16
+                                         returning 1 (every channel on the 12.5 kHz raster): the fast forms for any shape.
+                                         The row's shared work (the fold and 4-point split, and at taps > K the pre-sum) is
+                                         done once per row for all channels, and every channel's twiddles come from one
+                                         table per context.  At taps = K the envelope is bit-identical to
+                                         ACB_FLAG_FAST_CHANNELIZER's definition (the folded form, oracle
+                                         orc_channelize_dft8*), at taps > K to ACB_FLAG_FAST_FILTER's (the polyphase form),
+                                         with the same tolerances.  Where ACB_FLAG_FAST_CHANNELIZER or ACB_FLAG_FAST_FILTER
+                                         also applies (K = 160 or 192) their kernels run; the bits are the same.  Anything
+                                         else runs what runs without this flag: taps < K, acb_set_wf tables, a stream off the
+                                         raster, K % 8 != 0, real input (no effect).  ACB_FAST_FOLD8 does not apply. */
 #define ACB_FLAG_REAL_INPUT 2         /* Airspy front-end (air.c): float32 REAL samples at IF = rate/4,
                                          rate = K*12500; use acb_set_plan_air / acb_submit_real_host */
 
@@ -351,7 +364,8 @@ typedef struct {
 	double   demod_ms;          /* accumulated device time from a demod kernel's start to the end of its block FEC */
 	uint64_t chan_launches, demod_launches;
 	uint64_t fast_chan_launches; /* channelizer launches that took a fast form: ACB_FLAG_FAST_CHANNELIZER's (taps = K) or
-	                                ACB_FLAG_FAST_FILTER's or ACB_FLAG_FAST_FILTER_REAL's (taps > K) */
+	                                ACB_FLAG_FAST_FILTER's or ACB_FLAG_FAST_FILTER_REAL's (taps > K),
+	                                or ACB_FLAG_FAST_WIDEBAND's (either) */
 	uint64_t frames_lost;       /* frames that found the device ring full (ACB_ERR_OVERFLOW was returned once per submit) */
 	double   host_ms;           /* accumulated wall time the consumer thread spent ordering and queuing frames */
 } acb_stats_t;

@@ -62,4 +62,15 @@ with api.Context(Ka, 1, 3, 3, flags=2 | 8) as ctx:
         ctx.submit_real(part)
     ctx.sync()
     assert ctx.stats().fast_chan_launches >= 3
+# the wideband fast form at its largest shared-memory configuration (K = 1808: 12-row tiles, 115704 bytes per CTA),
+# taps > K, ragged CS16 submits
+Kw = 1808
+fw = [120_000_000 + 25_000 * (i // 2 + 1) * (1 if i % 2 == 0 else -1) for i in range(13)]
+xw = np.random.default_rng(1).integers(-32768, 32768, size=(1, 40 * Kw + 77, 2), dtype=np.int16)
+with api.Context(Kw, 1, 13, 1, flags=4 | api.FLAG_FAST_WIDEBAND, taps=2 * Kw + 3) as ctx:
+    ctx.set_plan_cs16(0, fw, 0, 120_000_000)
+    for part in (xw, xw[:, :1000], xw[:, :17 * Kw + 3]):
+        ctx.submit_cs16(part)
+    ctx.sync()
+    assert ctx.stats().fast_chan_launches == 2          # the 1000-sample submit completes no row
 print("sanitize run ok", n1, n3, n4, n5)
