@@ -255,6 +255,8 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	if (!cfg || !out) return fail(ACB_ERR_ARG, "null argument");
 	if (cfg->K < 1 || cfg->K > ACB_MAXK) return fail(ACB_ERR_ARG, "K=%d out of range 1..%d", cfg->K, ACB_MAXK);
 	if (cfg->nstreams < 1 || cfg->nch < 1 || cfg->max_blocks < 1) return fail(ACB_ERR_ARG, "nstreams/nch/max_blocks must be >= 1");
+	/* streams are grid.y of the channelizer launches (and of k_interleave_cs16), which CUDA caps at 65535 */
+	if (cfg->nstreams > ACB_MAXSTREAMS) return fail(ACB_ERR_ARG, "nstreams=%d exceeds %d", cfg->nstreams, ACB_MAXSTREAMS);
 	if (cfg->taps < 0 || cfg->taps > ACB_MAXTAPS_PER_K * cfg->K)
 		return fail(ACB_ERR_ARG, "taps=%d must be 0 (= K) or 1..%d*K=%d", cfg->taps, ACB_MAXTAPS_PER_K, ACB_MAXTAPS_PER_K * cfg->K);
 	if ((cfg->flags & ACB_FLAG_REAL_INPUT) && (cfg->flags & ACB_FLAG_CS16_INPUT)) return fail(ACB_ERR_ARG, "REAL_INPUT and CS16_INPUT are exclusive");

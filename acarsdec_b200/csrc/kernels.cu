@@ -2757,7 +2757,8 @@ k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsign
 {
 	__shared__ unsigned short s_crc[256];
 	__shared__ unsigned short s_syn[8 * FEC_SYN_BYTES];
-	/* the grid is sized for the busiest step (one thread per frame up to 75 776 frames, then a stride loop); CTAs
+	/* the grid is sized for the busiest step (one thread per frame up to 4 * SMs * 128 frames, 67 584 on a 132-SM H100,
+	 * then a stride loop; tests/test_gpu_scale.py runs more than two passes); CTAs
 	 * with no frame leave before building the tables */
 	if (blockIdx.x * blockDim.x >= min(ctl->count, cap)) return;
 	for (int b = threadIdx.x; b < 256; b += blockDim.x) {

@@ -29,6 +29,7 @@ extern "C" {
 #define ACB_OUTBLK 1024     /* rtl.c:49       RTLOUTBUFSZ: output samples per IQ block */
 #define ACB_TXTMAX 250      /* acarsdec.h:55  msgblk_t.txt */
 #define ACB_MAXK 2048       /* rtl.c:39 caps rtlMult at 320; wideband configs go beyond */
+#define ACB_MAXSTREAMS 65535 /* streams per context: they are grid.y of the channelizer launches (CUDA's limit) */
 
 enum {
 	ACB_OK = 0,
@@ -44,7 +45,9 @@ typedef struct acb_ctx acb_ctx_t;
 typedef struct {
 	int device;             /* CUDA ordinal */
 	int K;                  /* rtlMult: input rate = K*12500, taps == decimation (rtl.c:213-214) */
-	int nstreams;           /* independent IQ streams served by this context */
+	int nstreams;           /* independent IQ streams served by this context, 1..ACB_MAXSTREAMS (65535): every
+	                           channelizer launch puts the streams in grid.y, which CUDA limits to 65535, so
+	                           acb_create refuses more with ACB_ERR_ARG */
 	int nch;                /* channels per stream */
 	int max_blocks;         /* largest nblk a submit call may carry (sizes device staging) */
 	int flags;              /* ACB_FLAG_* */
@@ -380,7 +383,9 @@ int acb_get_stats(acb_ctx_t *ctx, acb_stats_t *out, int reset);
  *                             (one wide stream, configs 3/5); each device fetches the block over its own PCIe link.
  * Stream / channel indices in the API and in the messages are global; messages are merged into the reference's
  * emission order (block, stream, channel, time; rtl.c:357-360).  cfg->device is ignored, `devices` names the
- * CUDA ordinals (repeats allowed: two contexts on one GPU). */
+ * CUDA ordinals (repeats allowed: two contexts on one GPU).  ACB_MAXSTREAMS applies to each part: a stream split
+ * accepts up to ndev * 65535 streams (the parts differ by at most one stream), a channel split 65535; a part over the
+ * limit fails acb_multi_create with ACB_ERR_ARG. */
 typedef struct acb_multi acb_multi_t;
 enum { ACB_MULTI_SPLIT_STREAMS = 0, ACB_MULTI_SPLIT_CHANNELS = 1 };
 int  acb_multi_create(const acb_config_t *cfg, const int *devices, int ndev, int mode, acb_multi_t **out);
