@@ -449,10 +449,25 @@ class Context:
         _check(self.lib, self.lib.acb_set_plan_air(self.h, stream, f.ctypes.data, len(f), C.byref(fc)))
         return fc.value
 
-    def submit_real(self, x: np.ndarray) -> int:
-        """x: float32 (nstreams, nsamples) real samples; returns envelope samples produced per channel."""
-        assert x.dtype == np.float32 and x.ndim == 2 and x.shape[0] == self.nstreams and x.strides[1] == 4
-        return _check(self.lib, self.lib.acb_submit_real_host(self.h, x.ctypes.data, x.strides[0] // 4, x.shape[1]))
+    @staticmethod
+    def _stream_stride(a: np.ndarray, sample_bytes: int, stream_stride: int | None) -> int:
+        """Stream stride in samples: the array's row pitch (a view into wider rows keeps its pitch), which an explicit
+        `stream_stride` must agree with when there is more than one stream."""
+        # numpy may give a length-1 axis any stride: only the strides of axes longer than 1 say where the data is
+        assert a.shape[1] <= 1 or a.strides[1] == sample_bytes
+        assert a.shape[0] <= 1 or a.strides[0] % sample_bytes == 0
+        pitch = a.strides[0] // sample_bytes if a.shape[0] > 1 else a.shape[1]
+        if stream_stride is None:
+            return pitch
+        assert stream_stride >= a.shape[1] and (a.shape[0] == 1 or stream_stride == pitch)
+        return stream_stride
+
+    def submit_real(self, x: np.ndarray, stream_stride: int | None = None) -> int:
+        """x: float32 (nstreams, nsamples) real samples, rows contiguous; stream s starts stream_stride samples after
+        stream s-1 (default: the array's row pitch).  Returns envelope samples produced per channel."""
+        assert x.dtype == np.float32 and x.ndim == 2 and x.shape[0] == self.nstreams
+        stride = self._stream_stride(x, 4, stream_stride)
+        return _check(self.lib, self.lib.acb_submit_real_host(self.h, x.ctypes.data, stride, x.shape[1]))
 
     def set_plan_cs16(self, stream: int, freqs_hz, variant: int, fc_hz: int = 0) -> int:
         f = np.asarray(freqs_hz, dtype=np.uint32)
@@ -460,15 +475,20 @@ class Context:
         _check(self.lib, self.lib.acb_set_plan_cs16(self.h, stream, f.ctypes.data, len(f), variant, fc_hz, C.byref(fc)))
         return fc.value
 
-    def submit_cs16(self, iq: np.ndarray) -> int:
-        """iq: int16 (nstreams, nsamples, 2) interleaved I,Q."""
-        assert iq.dtype == np.int16 and iq.ndim == 3 and iq.shape[0] == self.nstreams and iq.shape[2] == 2 and iq.flags.c_contiguous
-        return _check(self.lib, self.lib.acb_submit_cs16_host(self.h, iq.ctypes.data, iq.shape[1], iq.shape[1]))
+    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None) -> int:
+        """iq: int16 (nstreams, nsamples, 2) interleaved I,Q, rows contiguous; stream_stride in complex samples
+        (default: the array's row pitch)."""
+        assert iq.dtype == np.int16 and iq.ndim == 3 and iq.shape[0] == self.nstreams and iq.shape[2] == 2 and iq.strides[2] == 2
+        stride = self._stream_stride(iq, 4, stream_stride)
+        return _check(self.lib, self.lib.acb_submit_cs16_host(self.h, iq.ctypes.data, stride, iq.shape[1]))
 
-    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray) -> int:
-        """xi, xq: int16 (nstreams, nsamples) separate I and Q planes (the SDRplay callback's layout)."""
-        assert xi.dtype == np.int16 and xq.dtype == np.int16 and xi.shape == xq.shape and xi.flags.c_contiguous and xq.flags.c_contiguous
-        return _check(self.lib, self.lib.acb_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, xi.shape[1], xi.shape[1]))
+    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None) -> int:
+        """xi, xq: int16 (nstreams, nsamples) separate I and Q planes (the SDRplay callback's layout), rows contiguous and
+        both planes with the same stream_stride (default: their row pitch)."""
+        assert xi.dtype == np.int16 and xq.dtype == np.int16 and xi.shape == xq.shape and xi.shape[0] == self.nstreams
+        stride = self._stream_stride(xi, 2, stream_stride)
+        assert self._stream_stride(xq, 2, stream_stride) == stride
+        return _check(self.lib, self.lib.acb_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, stride, xi.shape[1]))
 
     def set_emission_groups(self, unit: int, period: int = 0) -> None:
         """unit: 0 per submit, 1 every `period` envelope samples, 2 per transfer of `period` input samples."""

@@ -274,7 +274,9 @@ int acb_set_plan_cs16(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int 
  * the acb_build_wf_lp family's low-pass tables at taps > K; they fail with ACB_ERR_ARG at taps < K.
  * Same, with caller-supplied tables (nch x 2*taps floats; taps = K: e.g. taken from channel[].wf). */
 int acb_set_wf(acb_ctx_t *ctx, int stream, const float *wf, int nch);
-/* initMsk + initAcars for every channel of every stream (msk.c:30-51, acars.c:230-234). */
+/* initMsk + initAcars for every channel of every stream (msk.c:30-51, acars.c:230-234).  Submits still in flight
+ * are abandoned with their frames.  The streaming submits' carried remainder (the samples that did not fill a row)
+ * and the taps > K history are discarded: row 0 after a reset starts with the next sample submitted. */
 int acb_reset(acb_ctx_t *ctx);
 
 /* ---- processing ---- */
@@ -299,6 +301,13 @@ int acb_submit_real_host(acb_ctx_t *ctx, const float *x, size_t stream_stride_sa
  * carried (the reference carries ch->D and the tap index).  Returns envelope samples produced. */
 int acb_submit_cs16_host(acb_ctx_t *ctx, const int16_t *iq, size_t stream_stride_samples, size_t nsamples);
 int acb_submit_cs16_planar_host(acb_ctx_t *ctx, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples, size_t nsamples);
+/* Input lifetime, the three streaming calls (real, CS16, CS16 planar): the context copies what it needs (the carried
+ * remainder and history live on the device), so:
+ *   - pageable memory may be overwritten as soon as the call returns;
+ *   - pinned memory (acb_host_alloc) is read asynchronously.  It may be overwritten once an acb_collect or acb_sync has
+ *     covered the submit.  Submits that produced rows are covered in call order, one per acb_collect (the oldest first),
+ *     and all of them by acb_sync.  A submit that produced no row (returned 0) is covered only by the next acb_sync.
+ * A refused call (negative return) has read nothing, and the carried remainder is unchanged. */
 /* Emission order of the streaming front-ends (SURVEY H5).  The reference runs demodMSK channel by channel on
  * whatever a transfer (air.c:336) or a full dm_buffer (soapy.c:247: 1024 outputs; sdrplay.c:229: 512) delivered, so
  * its messages leave in (group, channel, time) order.  A submit may carry many such groups; tell the context how
