@@ -52,7 +52,7 @@ struct RingCtl {
 };
 
 /* channelizer tile geometry */
-constexpr int CH_TILE = 128;          /* threads per channelizer CTA (2 output rows each) */
+constexpr int CH_TILE = 128;          /* threads per two-row channelizer CTA (2 output rows each) */
 constexpr int CH_GROUP = 8;           /* channels accumulated per pass */
 
 /* wideband fast form (k_channelize_wb): channels per CTA, channel slots per thread, slot capacity per channel tile (every
@@ -111,7 +111,6 @@ int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_st
                            size_t nsamples, int nstreams, CUstream_st *stream);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
-size_t channelize_smem_bytes(int mode);
 } // namespace acb
 
 #endif

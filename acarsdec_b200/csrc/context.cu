@@ -87,7 +87,7 @@ struct acb_ctx {
 	cudaEvent_t ev_copied[2], ev_consumed[2];
 	bool buf_used[2];
 	int next_buf;
-	float *d_wf4;                /* [stream][grp][K][8] float4 (c, d, -d, c) */
+	float *d_wf;                 /* [stream][grp][taps_pad][8] float2 (c, d) */
 	bool fast;                   /* ACB_FLAG_FAST_CHANNELIZER and a shape k_channelize_dft takes */
 	bool fast_ovl;               /* taps > K and the polyphase form: ACB_FLAG_FAST_FILTER on u8 / CS16 with a K
 	                                k_channelize_ovl_fast takes, ACB_FLAG_FAST_FILTER_REAL on real input with a K
@@ -347,9 +347,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	/* u8 IQ history: its own buffer (acb_submit_device copies no input).  The streaming kinds keep theirs in front of
 	 * the carried remainder in d_real. */
 	if (c->hpad && !c->real_input) CU(cudaMalloc(&c->d_hist, (size_t)cfg->nstreams * c->hpad * 2));
-	const size_t wf_floats = (size_t)cfg->nstreams * c->ngrp * c->taps_pad * CH_GROUP * (c->in_kind == IN_KIND_F32REAL ? 2 : 4);
-	CU(cudaMalloc(&c->d_wf4, wf_floats * sizeof(float)));
-	CU(cudaMemsetAsync(c->d_wf4, 0, wf_floats * sizeof(float), c->s_copy));
+	const size_t wf_floats = (size_t)cfg->nstreams * c->ngrp * c->taps_pad * CH_GROUP * 2;
+	CU(cudaMalloc(&c->d_wf, wf_floats * sizeof(float)));
+	CU(cudaMemsetAsync(c->d_wf, 0, wf_floats * sizeof(float), c->s_copy));
 	CU(cudaStreamSynchronize(c->s_copy));
 	c->fast = (cfg->flags & ACB_FLAG_FAST_CHANNELIZER) && c->taps == cfg->K &&
 	          (c->in_kind == IN_KIND_F32REAL ? channelize_rdft_supports(cfg->K) : channelize_dft_supports(cfg->K));
@@ -466,7 +466,7 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 		if (c->ev_real_copied) cudaEventDestroy(c->ev_real_copied);
 		cudaFree(c->d_planar);
 		cudaFree(c->d_hist);
-		cudaFree(c->d_wf4); cudaFree(c->d_state);
+		cudaFree(c->d_wf); cudaFree(c->d_state);
 		cudaFree(c->d_tw); cudaFree(c->d_twmeta); cudaFree(c->d_p);
 		cudaFree(c->d_wbE); cudaFree(c->d_wbmeta);
 		for (int i = 0; i < NPIPE; i++) {
@@ -501,19 +501,17 @@ extern "C" int acb_set_wf(acb_ctx_t *c, int stream, const float *wf, int nch)
 	if (int r = ctx_use(c)) return r;
 	const int T = c->taps, TP = c->taps_pad;      /* taps beyond T keep zero weights: D + (+0) = D */
 	const int lead = c->hpad ? TP - T : 0;        /* taps > K: the padding goes in front (acb_create) */
-	const int W = c->in_kind == IN_KIND_F32REAL ? 2 : 4;
-	std::vector<float> t((size_t)c->ngrp * TP * CH_GROUP * W, 0.0f);
+	std::vector<float> t((size_t)c->ngrp * TP * CH_GROUP * 2, 0.0f);     /* (c, d) per (tap, channel), every input kind */
 	for (int ch = 0; ch < nch; ch++) {
 		const int g = ch / CH_GROUP, cc = ch % CH_GROUP;
 		for (int ind = 0; ind < T; ind++) {
 			const float re = wf[((size_t)ch * T + ind) * 2], im = wf[((size_t)ch * T + ind) * 2 + 1];
-			float *o = &t[(((size_t)g * TP + lead + ind) * CH_GROUP + cc) * W];
+			float *o = &t[(((size_t)g * TP + lead + ind) * CH_GROUP + cc) * 2];
 			o[0] = re; o[1] = im;
-			if (W == 4) { o[2] = -im; o[3] = re; }            /* (c, d, -d, c): see cmac() */
 		}
 	}
 	if (int r = sync_streams(c)) return r;
-	if (int r = upload(c, c->d_wf4 + (size_t)stream * t.size(), t.data(), t.size() * sizeof(float))) return r;
+	if (int r = upload(c, c->d_wf + (size_t)stream * t.size(), t.data(), t.size() * sizeof(float))) return r;
 	c->fast_ok[stream] = 0;                     /* a caller's table has no known structure: exact kernel */
 	return ACB_OK;
 }
@@ -886,15 +884,15 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			c->stats.kernel_launches++;
 			c->stats.fast_chan_launches++;
 		} else if (fast) {
-			r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp,
+			r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp,
 			                      hist, c->s_comp);
 			c->stats.kernel_launches++;
 		}
 		if (!r && !all_rows && nsamp > fast * OUTBLK) {
 			const size_t row0 = (size_t)fast * OUTBLK, nrows = (size_t)nsamp - row0;
-			r = c->hpad ? launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch,
+			r = c->hpad ? launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch,
 			                                            c->cfg.nstreams, row0, nrows, (size_t)nsamp, hist, c->s_comp)
-			            : launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
+			            : launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
 			                                        row0, nrows, (size_t)nsamp, c->s_comp);
 			c->stats.kernel_launches++;
 		}
@@ -905,7 +903,7 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
 			const unsigned long long lead = (H + K - 1) / K;
 			if (!r && fast && !ovl_fast && c->pos < lead) {
-				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf4, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
+				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
 				                                  0, (size_t)std::min<unsigned long long>(lead - c->pos, (unsigned long long)nsamp), (size_t)nsamp,
 				                                  hist, c->s_comp);
 				c->stats.kernel_launches++;

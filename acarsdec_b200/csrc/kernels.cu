@@ -66,13 +66,15 @@ __device__ __forceinline__ float2 cvt_iq(unsigned w, int pair)
 }
 
 /* D += (a + jb) * (c + jd) with the reference's rounding: products rounded, (ac - bd) and
- * (ad + bc) rounded, then the accumulate rounded (rtl.c:351).  w = (c, d, -d, c).
+ * (ad + bc) rounded, then the accumulate rounded (rtl.c:351).  w = (c, d).  The -bd product is
+ * b * (-d): negation is exact and round-to-nearest is symmetric, so it has the bits of a product with
+ * a stored -d, zero weights' signed zeros included; the negation folds into the FMUL's operand.
  * Instruction shape: 4 FMUL + 4 FADD, none of them contracted into an FFMA (that would skip the
  * product rounding). */
-__device__ __forceinline__ void cmac(float2 &acc, float a, float b, const float4 w)
+__device__ __forceinline__ void cmac(float2 &acc, float a, float b, const float2 w)
 {
 	const float2 p1 = fmul2_rn(make_float2(a, a), make_float2(w.x, w.y));
-	const float2 p2 = fmul2_rn(make_float2(b, b), make_float2(w.z, w.w));
+	const float2 p2 = fmul2_rn(make_float2(b, b), make_float2(-w.y, w.x));
 	const float2 t = make_float2(__fadd_rn(p1.x, p2.x), __fadd_rn(p1.y, p2.y));
 	acc = fadd2_rn(acc, t);
 }
@@ -93,30 +95,27 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 /* ------------------------------------------------------------------------------------------
- * K1 pipeline.  One CTA = one 1024-output block x one group of 8 channels; 128 threads, two
- * output rows per thread (rows t and t+128 of a 256-row tile) so every broadcast table load
- * feeds two complex MACs; the K taps are walked in chunks of 5 sixteen-byte units per row
- * (5 is odd: the strided LDS.128 row reads are conflict free without padding) staged by
- * cp.async into a 2-deep ring together with the matching slice of the table, so the copy of
- * chunk i+1 runs under the arithmetic of chunk i.  Any K that keeps rows 16-byte aligned, up to
- * ACB_MAXK.  MODE: u8 IQ with table entries (c, d, -d, c) (rtl.c:334-354); float32 real samples,
- * D += wf[i]*S, entries (c, d) (air.c:314-333); CS16 IQ, same complex MAC as u8 on (float)int16
- * (soapy.c:239-242 with the /32768.0 folded into the table, sdrplay.c:218-222).
+ * K1 pipeline, float32 real input (air.c:314-333: D += wf[i]*S, table entries (c, d)), the two-rows form that
+ * ACB_REAL_ROWS=2 selects in place of k_channelize_real4.  One CTA = one 1024-output block x one group of 8 channels;
+ * 128 threads, two output rows per thread (rows t and t+128 of a 256-row tile) so every broadcast table load feeds two
+ * MACs; the K taps are walked in chunks of 5 sixteen-byte units per row (5 is odd: the strided LDS.128 row reads are
+ * conflict free without padding) staged by cp.async into a 2-deep ring together with the matching slice of the table,
+ * so the copy of chunk i+1 runs under the arithmetic of chunk i.  Any K that keeps rows 16-byte aligned, up to ACB_MAXK.
  * ---------------------------------------------------------------------------------------- */
 
 constexpr int C2_ROWS = 256;
 enum { IN_U8IQ = 0, IN_F32REAL = 1, IN_CS16IQ = 2 };   /* input sample formats (acb_internal.h: InputKind) */
 
-template <int MODE> struct C2 {
+struct C2 {
 	/* 16-byte units of a row per chunk: odd, so the strided per-thread LDS.128 row reads are conflict free with rows
-	 * packed back to back.  (Whole-sector chunks of 6 units with a padded row stride were tried for the 4-byte-per-tap
-	 * inputs: no gain — their limit was elsewhere, see k_channelize_real4.) */
+	 * packed back to back.  (Whole-sector chunks of 6 units with a padded row stride were tried: no gain — the limit
+	 * was elsewhere, see k_channelize_real4.) */
 	static constexpr int UNITS = 5;
 	static constexpr int ROW_UNITS = UNITS;                      /* shared-memory row stride in units */
 	static constexpr int STAGES = 2;                             /* cp.async ring depth */
-	static constexpr int TAP_BYTES = MODE == IN_U8IQ ? 2 : 4;    /* input bytes per tap */
+	static constexpr int TAP_BYTES = 4;                          /* input bytes per tap */
 	static constexpr int TAPS_PER_UNIT = 16 / TAP_BYTES;
-	static constexpr int W_BYTES = MODE == IN_F32REAL ? 8 : 16;  /* table bytes per (tap, channel) */
+	static constexpr int W_BYTES = 8;                            /* table bytes per (tap, channel) */
 	static constexpr int CHUNK_TAPS = UNITS * TAPS_PER_UNIT;
 	static constexpr int TILE_BYTES = C2_ROWS * ROW_UNITS * 16;
 	static constexpr int WF_BYTES = CHUNK_TAPS * CH_GROUP * W_BYTES;
@@ -144,13 +143,13 @@ __device__ __forceinline__ void rmac(float2 &acc, float sv, const float2 w)
  * the row and is `taps` (= K + H_pad) samples long.  A 16-byte unit that lies before the stream's input of this submit
  * is fetched from the history of the stream instead: `hist + s*hist_stride + hbytes` is where sample 0 of the submit
  * would sit if the history were laid out in front of it.  The choice is per unit: H_pad and every row are whole units. */
-template <int MODE, bool OVL>
+template <bool OVL>
 __global__ void __launch_bounds__(CH_TILE)
 k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t *__restrict__ wf,
               float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp,
               const uint8_t *__restrict__ hist, size_t hist_stride, int hbytes)
 {
-	using T = C2<MODE>;
+	using T = C2;
 	extern __shared__ __align__(16) unsigned char smem[];
 	const int t = threadIdx.x;
 	const int blk = blockIdx.x, s = blockIdx.y;
@@ -220,44 +219,15 @@ k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t
 			for (int j = 0; j < uc; j++) {
 				const uint4 qa = rowA[j], qb = rowB[j];
 				const unsigned wa[4] = { qa.x, qa.y, qa.z, qa.w }, wb[4] = { qb.x, qb.y, qb.z, qb.w };
-				if (MODE == IN_F32REAL) {
-					const float2 *wj = reinterpret_cast<const float2 *>(st + T::TILE_BYTES) + (size_t)j * 4 * CH_GROUP;
+				const float2 *wj = reinterpret_cast<const float2 *>(st + T::TILE_BYTES) + (size_t)j * 4 * CH_GROUP;
 #pragma unroll
-					for (int e = 0; e < 4; e++) {
-						const float sa = __uint_as_float(wa[e]), sb = __uint_as_float(wb[e]);
+				for (int e = 0; e < 4; e++) {
+					const float sa = __uint_as_float(wa[e]), sb = __uint_as_float(wb[e]);
 #pragma unroll
-						for (int c = 0; c < CH_GROUP; c++) {
-							const float2 w = wj[e * CH_GROUP + c];
-							rmac(accA[c], sa, w);
-							rmac(accB[c], sb, w);
-						}
-					}
-				} else if (MODE == IN_CS16IQ) {
-					const float4 *wj = reinterpret_cast<const float4 *>(st + T::TILE_BYTES) + (size_t)j * 4 * CH_GROUP;
-#pragma unroll
-					for (int e = 0; e < 4; e++) {
-						const float2 xa = cvt_cs16(wa[e]), xb = cvt_cs16(wb[e]);
-#pragma unroll
-						for (int c = 0; c < CH_GROUP; c++) {
-							const float4 w = wj[e * CH_GROUP + c];
-							cmac(accA[c], xa.x, xa.y, w);
-							cmac(accB[c], xb.x, xb.y, w);
-						}
-					}
-				} else {
-					const float4 *wj = reinterpret_cast<const float4 *>(st + T::TILE_BYTES) + (size_t)j * 8 * CH_GROUP;
-#pragma unroll
-					for (int e = 0; e < 4; e++) {
-#pragma unroll
-						for (int h = 0; h < 2; h++) {
-							const float2 xa = cvt_iq(wa[e], h), xb = cvt_iq(wb[e], h);
-#pragma unroll
-							for (int c = 0; c < CH_GROUP; c++) {
-								const float4 w = wj[(2 * e + h) * CH_GROUP + c];
-								cmac(accA[c], xa.x, xa.y, w);
-								cmac(accB[c], xb.x, xb.y, w);
-							}
-						}
+					for (int c = 0; c < CH_GROUP; c++) {
+						const float2 w = wj[e * CH_GROUP + c];
+						rmac(accA[c], sa, w);
+						rmac(accB[c], sb, w);
 					}
 				}
 			}
@@ -281,6 +251,132 @@ k_channelize(const uint8_t *__restrict__ in, size_t stream_stride, const uint8_t
 				}
 			}
 			__syncthreads();                                         /* stage may be refilled by issue(step+2) */
+		}
+	}
+}
+
+/* ------------------------------------------------------------------------------------------
+ * K1 for IQ input: u8 (rtl.c:334-354) and CS16 (soapy.c:239-242 with the /32768.0 folded into the table,
+ * sdrplay.c:218-222), D += (a + jb)(c + jd) per tap in tap order (cmac).
+ *
+ * One CTA = 512 output rows (half a 1024-row block) x one group of 8 channels; 128 threads, FOUR rows per thread (rows
+ * t + 128 r), so each warp-uniform LDS.128 of the table — (c, d) of two channels — feeds 4 rows x 2 channels = 8 complex
+ * MACs.  The instruction stream is the FP32 pipe's: per 32-bit word of the rows (u8: 2 taps) and thread, 64 complex MACs
+ * = 512 FMUL/FADD, 48 conversion instructions and 8 table loads.
+ *
+ * Only the table goes through shared memory, in a 2-deep cp.async ring of IQ4_CU-unit chunks (2 x 2 KB for u8, 2 x 1 KB
+ * for CS16, whatever K or taps): K1 then fits on an SM beside the co-resident demodulator's CTAs.  Each thread loads its
+ * rows' 16-byte units straight from global memory into registers (qb), one unit ahead of the arithmetic on qa.  The two
+ * units of a 32-byte sector are consecutive loads of the same thread, so DRAM is read once.  OVL: the window and the
+ * per-unit choice between input and history are those of k_channelize.
+ * ---------------------------------------------------------------------------------------- */
+constexpr int IQ4_THREADS = 128, IQ4_RPT = 4, IQ4_ROWS = IQ4_THREADS * IQ4_RPT;
+constexpr int IQ4_CU = 4;            /* table chunk in units of the row */
+constexpr int IQ4_STAGES = 2;
+
+template <int MODE, bool OVL>
+__global__ void __launch_bounds__(IQ4_THREADS, 3)
+k_channelize_iq4(const uint8_t *__restrict__ in, size_t stream_stride, const float2 *__restrict__ wf,
+                 float *__restrict__ dm, int K, int taps, int nch, int ngrp, size_t nsamp,
+                 const uint8_t *__restrict__ hist, size_t hist_stride, int hbytes)
+{
+	constexpr int TB = MODE == IN_U8IQ ? 2 : 4, TPU = 16 / TB;        /* input bytes per tap, taps per unit */
+	constexpr int TPW = TPU / 4;                                       /* taps per 32-bit word */
+	constexpr int WCH = IQ4_CU * TPU * CH_GROUP;                       /* (c, d) entries per table chunk */
+	__shared__ __align__(16) float2 wsm[IQ4_STAGES][WCH];
+	const int t = threadIdx.x, s = blockIdx.y, g = blockIdx.z;
+	const size_t rowbytes = (size_t)K * TB;
+	const int U = taps / TPU;                                          /* units of each row's window (taps padded to whole units) */
+	const int nchunk = (U + IQ4_CU - 1) / IQ4_CU;
+	const size_t m0 = (size_t)blockIdx.x * IQ4_ROWS + t;               /* the thread's rows: m0 + 128 r */
+	const uint8_t *sbase = in + (size_t)s * stream_stride;
+	const uint8_t *hbase = OVL ? hist + (size_t)s * hist_stride + hbytes : nullptr;
+	const float2 *wsrc = wf + ((size_t)s * ngrp + g) * taps * CH_GROUP;
+	const uint8_t *rp[IQ4_RPT];                                        /* the rows' unit under the arithmetic */
+#pragma unroll
+	for (int r = 0; r < IQ4_RPT; r++) rp[r] = sbase + (m0 + (size_t)r * IQ4_THREADS) * rowbytes - (OVL ? hbytes : 0);
+
+	auto issue = [&](int ck) {                                         /* table chunk ck into its stage; always one commit */
+		if (ck < nchunk) {
+			const int n = min(IQ4_CU, U - ck * IQ4_CU) * TPU * CH_GROUP / 2;
+			const float2 *src = wsrc + (size_t)ck * WCH;
+			for (int i = t; i < n; i += IQ4_THREADS) cp_async16(&wsm[ck % IQ4_STAGES][2 * i], src + 2 * i);
+		}
+		cp_async_commit();
+	};
+	auto load = [&](uint4 (&q)[IQ4_RPT], int off) {                    /* the rows' unit at byte `off` past rp */
+#pragma unroll
+		for (int r = 0; r < IQ4_RPT; r++) {
+			const uint8_t *p = rp[r] + off;
+			if (OVL && p < sbase) p = hbase - (sbase - p);
+			q[r] = __ldg(reinterpret_cast<const uint4 *>(p));
+		}
+	};
+
+	float2 acc[IQ4_RPT][CH_GROUP];
+#pragma unroll
+	for (int r = 0; r < IQ4_RPT; r++)
+#pragma unroll
+		for (int c = 0; c < CH_GROUP; c++) acc[r][c] = make_float2(0.f, 0.f);
+
+	auto word = [&](const unsigned (&v)[IQ4_RPT], const float2 *wj) {    /* the TPW taps of one 32-bit word of the rows */
+#pragma unroll
+		for (int h = 0; h < TPW; h++) {
+			float2 x[IQ4_RPT];
+#pragma unroll
+			for (int r = 0; r < IQ4_RPT; r++) x[r] = MODE == IN_U8IQ ? cvt_iq(v[r], h) : cvt_cs16(v[r]);
+			const float4 *wt = reinterpret_cast<const float4 *>(wj + h * CH_GROUP);
+#pragma unroll
+			for (int c2 = 0; c2 < CH_GROUP / 2; c2++) {
+				const float4 w = wt[c2];
+#pragma unroll
+				for (int r = 0; r < IQ4_RPT; r++) {
+					cmac(acc[r][2 * c2], x[r].x, x[r].y, make_float2(w.x, w.y));
+					cmac(acc[r][2 * c2 + 1], x[r].x, x[r].y, make_float2(w.z, w.w));
+				}
+			}
+		}
+	};
+
+	uint4 qa[IQ4_RPT], qb[IQ4_RPT];
+	issue(0);
+	load(qa, 0);
+	int u = 0;                                                         /* unit in qa */
+	for (int ck = 0; ck < nchunk; ck++) {
+		issue(ck + 1);
+		asm volatile("cp.async.wait_group 1;" ::: "memory");
+		__syncthreads();                                               /* chunk ck visible to all */
+		const float2 *w = wsm[ck % IQ4_STAGES];
+		const int uc = min(IQ4_CU, U - ck * IQ4_CU);
+		/* rolled loops over units and over the 4 words of a unit: a body of one word (~580 instructions) stays in the
+		 * instruction cache, where a fully unrolled unit (~2300) or unit pair did not and ran 1.2x / 1.6x slower */
+#pragma unroll 1
+		for (int j = 0; j < uc; j++, u++) {
+			if (u + 1 < U) load(qb, 16);
+#pragma unroll 1
+			for (int e = 0; e < 4; e++, w += TPW * CH_GROUP) {
+				const unsigned v[IQ4_RPT] = { qa[0].x, qa[1].x, qa[2].x, qa[3].x };
+				word(v, w);
+#pragma unroll
+				for (int r = 0; r < IQ4_RPT; r++) { qa[r].x = qa[r].y; qa[r].y = qa[r].z; qa[r].z = qa[r].w; }
+			}
+#pragma unroll
+			for (int r = 0; r < IQ4_RPT; r++) { qa[r] = qb[r]; rp[r] += 16; }
+		}
+		__syncthreads();                                               /* stage may be refilled by issue(ck + 2) */
+	}
+
+	const int nc = min(CH_GROUP, nch - g * CH_GROUP);
+#pragma unroll
+	for (int r = 0; r < IQ4_RPT; r++) {
+		float *o = dm + ((size_t)s * nsamp + m0 + (size_t)r * IQ4_THREADS) * nch + g * CH_GROUP;
+		if (nc == CH_GROUP && (nch & 3) == 0) {
+			reinterpret_cast<float4 *>(o)[0] = make_float4(envelope(acc[r][0]), envelope(acc[r][1]), envelope(acc[r][2]), envelope(acc[r][3]));
+			reinterpret_cast<float4 *>(o)[1] = make_float4(envelope(acc[r][4]), envelope(acc[r][5]), envelope(acc[r][6]), envelope(acc[r][7]));
+		} else {
+#pragma unroll
+			for (int c = 0; c < CH_GROUP; c++)
+				if (c < nc) o[c] = envelope(acc[r][c]);
 		}
 	}
 }
@@ -412,31 +508,43 @@ static int launch_channelize_real4(const void *in, size_t stream_stride, const v
 	return (int)cudaGetLastError();
 }
 
-size_t channelize_smem_bytes(int mode)
-{
-	return mode == IN_F32REAL ? (size_t)C2<IN_F32REAL>::STAGES * C2<IN_F32REAL>::STAGE_BYTES
-	       : mode == IN_CS16IQ ? (size_t)C2<IN_CS16IQ>::STAGES * C2<IN_CS16IQ>::STAGE_BYTES
-	                           : (size_t)C2<IN_U8IQ>::STAGES * C2<IN_U8IQ>::STAGE_BYTES;
-}
-
-template <int MODE, bool OVL>
-static int launch_channelize_t(const void *in, size_t stream_stride, const void *wf, float *dm,
-                               int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
+template <bool OVL>
+static int launch_channelize_real2(const void *in, size_t stream_stride, const void *wf, float *dm,
+                                   int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
 {
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
-	const size_t smem = (size_t)C2<MODE>::STAGES * C2<MODE>::STAGE_BYTES;
-	cudaError_t e = cudaFuncSetAttribute(k_channelize<MODE, OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	const size_t smem = (size_t)C2::STAGES * C2::STAGE_BYTES;
+	cudaError_t e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) return (int)e;
 	/* both kernels ask for the largest shared-memory carve-out: an SM's L1/shared split only
 	 * changes when the SM is idle, so kernels that prefer different splits cannot be co-resident
 	 * — and the demod of submit i is meant to run underneath the channelizer of submit i+1 */
-	e = cudaFuncSetAttribute(k_channelize<MODE, OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 	if (e != cudaSuccess) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
-	k_channelize<MODE, OVL><<<grid, CH_TILE, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
-	                                                         reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
-	                                                         reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad * C2<MODE>::TAP_BYTES);
+	k_channelize<OVL><<<grid, CH_TILE, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
+	                                                   reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
+	                                                   reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad * C2::TAP_BYTES);
+	return (int)cudaGetLastError();
+}
+
+template <int MODE, bool OVL>
+static int launch_channelize_iq4(const void *in, size_t stream_stride, const float *wf, float *dm,
+                                 int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
+{
+	if (nblk == 0) return 0;
+	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
+	/* a quarter of the shared-memory maximum, the rest L1: every lane of a row load touches its own 128-byte line, and
+	 * with the 28 KB of L1 the largest carve-out leaves, the kernel ran 1.2x slower (DESIGN.md §4).  The demodulator's
+	 * CTAs still fit beside it (5 KB per K1 CTA). */
+	cudaError_t e = cudaFuncSetAttribute(k_channelize_iq4<MODE, OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, 25);
+	if (e != cudaSuccess) return (int)e;
+	dim3 grid(nblk * (OUTBLK / IQ4_ROWS), nstreams, ngrp);
+	k_channelize_iq4<MODE, OVL><<<grid, IQ4_THREADS, 0, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
+	                                                             reinterpret_cast<const float2 *>(wf), dm, K, taps, nch, ngrp, nsamp,
+	                                                             reinterpret_cast<const uint8_t *>(h.base), h.stride,
+	                                                             h.hpad * (MODE == IN_U8IQ ? 2 : 4));
 	return (int)cudaGetLastError();
 }
 
@@ -447,11 +555,11 @@ static int launch_channelize_k(int mode, const void *in, size_t stream_stride_by
 	switch (mode) {
 	case IN_F32REAL: {
 		const bool two_rows = getenv("ACB_REAL_ROWS") && atoi(getenv("ACB_REAL_ROWS")) == 2;     /* A/B switch: the 2-rows-per-thread form */
-		return two_rows ? launch_channelize_t<IN_F32REAL, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream)
+		return two_rows ? launch_channelize_real2<OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream)
 		                : launch_channelize_real4<OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
 	}
-	case IN_CS16IQ: return launch_channelize_t<IN_CS16IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
-	default: return launch_channelize_t<IN_U8IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
+	case IN_CS16IQ: return launch_channelize_iq4<IN_CS16IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
+	default: return launch_channelize_iq4<IN_U8IQ, OVL>(in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
 	}
 }
 
@@ -2135,21 +2243,21 @@ k_channelize_generic(const uint8_t *__restrict__ in, size_t stream_stride, const
 		}
 	} else if (MODE == IN_CS16IQ) {
 		const short *p = reinterpret_cast<const short *>(in + (size_t)s * stream_stride) + m * K * 2;
-		const float4 *w = reinterpret_cast<const float4 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
+		const float2 *w = reinterpret_cast<const float2 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
 		for (int ind = 0; ind < taps; ind++) {
 			const float a = (float)p[2 * ind], b = (float)p[2 * ind + 1];
-			const float4 ww = w[(size_t)ind * CH_GROUP];
-			dr = __fadd_rn(dr, __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, ww.z)));
-			di = __fadd_rn(di, __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.w)));
+			const float2 ww = w[(size_t)ind * CH_GROUP];
+			dr = __fadd_rn(dr, __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, -ww.y)));
+			di = __fadd_rn(di, __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.x)));
 		}
 	} else {
 		const uint8_t *p = in + (size_t)s * stream_stride + m * K * 2;
-		const float4 *w = reinterpret_cast<const float4 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
+		const float2 *w = reinterpret_cast<const float2 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
 		for (int ind = 0; ind < taps; ind++) {
 			float a = __fadd_rn((float)p[2 * ind], -127.37f), b = __fadd_rn((float)p[2 * ind + 1], -127.37f);
-			float4 ww = w[(size_t)ind * CH_GROUP];
-			float pr = __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, ww.z));
-			float pi = __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.w));
+			float2 ww = w[(size_t)ind * CH_GROUP];
+			float pr = __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, -ww.y));
+			float pi = __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.x));
 			dr = __fadd_rn(dr, pr);
 			di = __fadd_rn(di, pi);
 		}
@@ -2203,7 +2311,7 @@ k_channelize_generic_ovl(const uint8_t *__restrict__ in, size_t stream_stride, c
 			di = __fadd_rn(di, __fmul_rn(ww.y, x));
 		}
 	} else {
-		const float4 *w = reinterpret_cast<const float4 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
+		const float2 *w = reinterpret_cast<const float2 *>(wf) + ((size_t)s * ngrp + ch / CH_GROUP) * taps * CH_GROUP + (ch % CH_GROUP);
 		for (int i = first; i < taps; i++) {
 			const long long o = o0 + i;
 			const uint8_t *q = o < 0 ? hp + o * TB : p + o * TB;
@@ -2215,9 +2323,9 @@ k_channelize_generic_ovl(const uint8_t *__restrict__ in, size_t stream_stride, c
 				a = __fadd_rn((float)q[0], -127.37f);
 				b = __fadd_rn((float)q[1], -127.37f);
 			}
-			const float4 ww = w[(size_t)i * CH_GROUP];
-			dr = __fadd_rn(dr, __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, ww.z)));
-			di = __fadd_rn(di, __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.w)));
+			const float2 ww = w[(size_t)i * CH_GROUP];
+			dr = __fadd_rn(dr, __fadd_rn(__fmul_rn(a, ww.x), __fmul_rn(b, -ww.y)));
+			di = __fadd_rn(di, __fadd_rn(__fmul_rn(a, ww.y), __fmul_rn(b, ww.x)));
 		}
 	}
 	dm[((size_t)s * nsamp + m) * nch + ch] = envelope(make_float2(dr, di));
