@@ -18,6 +18,7 @@ LIB_PATH = PKG / "libacars_b200.so"
 OUTBLK = 1024
 TXTMAX = 250
 FLAG_FAST_WIDEBAND = 64          # ACB_FLAG_FAST_WIDEBAND: the fast forms for any K % 8 == 0 and any channel count
+FLAG_FAST_WIDEBAND_REAL = 128    # ACB_FLAG_FAST_WIDEBAND_REAL: the same for real input (air.c)
 
 
 class Config(C.Structure):

@@ -66,7 +66,9 @@ constexpr int WB_META = 2 + 2 * WB_SLOTS;
 } // namespace acb
 
 /* hostmath.cpp: the wideband form's twiddle table E[r + K - 1], r in (-K, K), with the fast planners' expression for the
- * exponent r = (k*n2) % K; variant -1: u8 (acb_fast_plan), else a CS16 variant (acb_fast_plan_cs16).  1 on success. */
+ * exponent r = (k*n2) % K; variant -1: u8 (acb_fast_plan), ACB_WB_TW_REAL: real input (acb_fast_plan_air, K % 8 == 0),
+ * else a CS16 variant (acb_fast_plan_cs16).  1 on success. */
+#define ACB_WB_TW_REAL 2
 extern "C" int acb_wb_twiddles(int variant, int K, float *E);
 
 /* kernels.cu entry points (host-callable launchers) */
@@ -106,6 +108,8 @@ int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw
                            int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
                                const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
+int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
+                              float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
 int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_stride, uint32_t *out, size_t out_stride,
                            size_t nsamples, int nstreams, CUstream_st *stream);

@@ -92,8 +92,9 @@ struct acb_ctx {
 	bool fast_ovl;               /* taps > K and the polyphase form: ACB_FLAG_FAST_FILTER on u8 / CS16 with a K
 	                                k_channelize_ovl_fast takes, ACB_FLAG_FAST_FILTER_REAL on real input with a K
 	                                k_channelize_ovl_rdft takes */
-	bool wb;                     /* ACB_FLAG_FAST_WIDEBAND on u8 / CS16, K % 8 == 0, taps >= K, and neither of the
-	                                above selects a narrow kernel: k_channelize_wb */
+	bool wb;                     /* ACB_FLAG_FAST_WIDEBAND on u8 / CS16 (k_channelize_wb) or ACB_FLAG_FAST_WIDEBAND_REAL on
+	                                real input (k_channelize_wb_real), K % 8 == 0, taps >= K, and neither of the above
+	                                selects a narrow kernel */
 	float *d_wbE;                /* wb: the twiddle table(s) E of acb_wb_twiddles, 2K - 1 (Tr, Ti) each; CS16: one per variant */
 	int *d_wbmeta;               /* wb: [stream][channel tile][WB_META] residue-sorted slots (upload_wb_plan) */
 	float *d_p;                  /* fast_ovl, wb at taps > K: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
@@ -356,8 +357,8 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->fast_ovl = c->taps > cfg->K &&
 	              (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_FILTER_REAL) && channelize_rdft_supports(cfg->K)
 	                                             : (cfg->flags & ACB_FLAG_FAST_FILTER) && channelize_dft_supports(cfg->K));
-	c->wb = (cfg->flags & ACB_FLAG_FAST_WIDEBAND) && c->in_kind != IN_KIND_F32REAL && cfg->K % 8 == 0 && c->taps >= cfg->K &&
-	        !c->fast && !c->fast_ovl;
+	c->wb = (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_WIDEBAND_REAL) : (cfg->flags & ACB_FLAG_FAST_WIDEBAND)) &&
+	        cfg->K % 8 == 0 && c->taps >= cfg->K && !c->fast && !c->fast_ovl;
 	c->d_wbE = nullptr;
 	c->d_wbmeta = nullptr;
 	c->d_p = nullptr;
@@ -385,7 +386,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		const size_t per = (size_t)(2 * cfg->K - 1) * 2;
 		std::vector<float> E(ntab * per);
 		for (int t = 0; t < ntab; t++)
-			acb_wb_twiddles(c->in_kind == IN_KIND_CS16IQ ? t : -1, cfg->K, &E[t * per]);
+			acb_wb_twiddles(c->in_kind == IN_KIND_CS16IQ ? t : c->in_kind == IN_KIND_F32REAL ? ACB_WB_TW_REAL : -1, cfg->K, &E[t * per]);
 		CU(cudaMalloc(&c->d_wbE, E.size() * sizeof(float)));
 		if (int r = upload(c, c->d_wbE, E.data(), E.size() * sizeof(float))) return r;
 		const size_t nct = (size_t)(cfg->nch + WB_CTILE - 1) / WB_CTILE;
@@ -536,20 +537,23 @@ static int upload_fast_plan(acb_ctx *c, int stream, bool ok, const std::vector<i
 	return ACB_OK;
 }
 
-/* wideband form: per channel tile, the channel slots sorted by bin residue (k/2) mod 4 and each residue class padded to
- * whole groups of WB_CB (channel -1), so that every thread of k_channelize_wb multiplies one Y' row; `etab` selects the
- * twiddle table (CS16: the variant).  `ok` false leaves the stream on the exact kernel. */
+/* wideband form: per channel tile, the channel slots sorted by bin residue (k/2) mod 4 (real input: by the column the
+ * real form reads, k mod 4 = 0, 2 or odd) and each class padded to whole groups of WB_CB (channel -1), so that every
+ * thread of k_channelize_wb(_real) multiplies one Y' column; `etab` selects the twiddle table (CS16: the variant).  `ok`
+ * false leaves the stream on the exact kernel. */
 static int upload_wb_plan(acb_ctx *c, int stream, bool ok, const std::vector<int> &kbin, int etab)
 {
 	if (!ok) return ACB_OK;
 	const int nch = c->cfg.nch, nct = (nch + WB_CTILE - 1) / WB_CTILE;
+	const bool real = c->in_kind == IN_KIND_F32REAL;
+	auto cls = [real](int k) { return real ? ((k & 3) == 0 ? 0 : (k & 3) == 2 ? 1 : 2) : (((k / 2) % 4) + 4) % 4; };
 	std::vector<int> meta((size_t)nct * WB_META, 0);
 	for (int z = 0; z < nct; z++) {
 		int *m = &meta[(size_t)z * WB_META];
 		int slot = 0;
 		for (int res = 0; res < 4; res++) {
 			for (int ch = z * WB_CTILE; ch < std::min(nch, (z + 1) * WB_CTILE); ch++) {
-				if ((((kbin[ch] / 2) % 4) + 4) % 4 != res) continue;
+				if (cls(kbin[ch]) != res) continue;
 				m[2 + 2 * slot] = kbin[ch];
 				m[3 + 2 * slot] = ch;
 				slot++;
@@ -846,7 +850,15 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			hist.base = d_iq - (size_t)c->hpad * 4;
 			hist.stride = stride;
 		}
-		if (dft && c->wb) {
+		if (dft && c->wb && c->in_kind == IN_KIND_F32REAL) {
+			/* every row of the submit; at taps > K the history sits right in front of each stream's rows in d_real
+			 * (submit4), zeros after create / reset */
+			r = launch_channelize_wb_real(d_iq, stride, c->hpad, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                              c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			c->stats.kernel_launches++;
+			c->stats.fast_chan_launches++;
+			all_rows = true;
+		} else if (dft && c->wb) {
 			/* every row of the submit, CS16 partial blocks included; at taps > K the terms before the stream start are
 			 * omitted in the kernel */
 			r = launch_channelize_wb(c->in_kind, d_iq, stride, hist, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
@@ -1164,8 +1176,9 @@ extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_
 	}
 	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<int> kbin(nch);
+	if (c->wb) return upload_wb_plan(c, stream, acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), nullptr) == 1, kbin, 0);
+	if (!c->fast && !c->fast_ovl) return ACB_OK;
 	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
 	const bool ok = acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;
 	return upload_fast_plan(c, stream, ok, kbin, tw1);

@@ -313,9 +313,12 @@ extern "C" int acb_wb_twiddles(int variant, int K, float *E)
 {
 	/* Every twiddle the two planners above write depends on k and n2 only through r = (k*n2) % K (C remainder: the sign of
 	 * k), so one table indexed by r in (-K, K) serves every channel of a context (k_channelize_wb).  Both signs are kept:
-	 * cos(2*pi*(r + K)/K) need not round like cos(2*pi*r/K).  The expressions are the planners' own, token for token. */
+	 * cos(2*pi*(r + K)/K) need not round like cos(2*pi*r/K).  The expressions are the planners' own, token for token.
+	 * Real input (acb_fast_plan_air below, k_channelize_wb_real): 0 < k < K, so only r in [0, K) occurs; the table keeps
+	 * the same layout. */
 	if (!E || K <= 0 || K > ACB_MAXK || (K & 3)) return 0;
-	if (variant != -1 && variant != ACB_CS16_SOAPY && variant != ACB_CS16_SDRPLAY) return 0;
+	if (variant != -1 && variant != ACB_CS16_SOAPY && variant != ACB_CS16_SDRPLAY && variant != ACB_WB_TW_REAL) return 0;
+	if (variant == ACB_WB_TW_REAL && (K & 7)) return 0;
 	const double scale = variant == ACB_CS16_SOAPY ? 1.0 / 32768.0 : 0.25;
 	for (int r = -(K - 1); r < K; r++) {
 		const double ph = -2.0 * M_PI * (double)r / (double)K;
@@ -323,6 +326,9 @@ extern "C" int acb_wb_twiddles(int variant, int K, float *E)
 		if (variant == -1) {
 			o[0] = (float)(cos(ph) / K / 127.5);
 			o[1] = (float)(sin(ph) / K / 127.5);
+		} else if (variant == ACB_WB_TW_REAL) {
+			o[0] = (float)(cos(ph) / K);
+			o[1] = (float)(sin(ph) / K);
 		} else {
 			o[0] = (float)(cos(ph) / K * scale);
 			o[1] = (float)(sin(ph) / K * scale);

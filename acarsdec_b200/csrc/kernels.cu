@@ -1583,6 +1583,17 @@ static int wb_rb(int K)
 	return 16 * 3 * K + (2 * K - 1) * 8 <= 113 * 1024 ? 3 : 2;
 }
 
+/* tiles per CTA of the wideband kernels (k_channelize_wb, k_channelize_wb_real): up to 8 (E is staged once per CTA), fewer
+ * where that would leave less than four waves of two CTAs per SM — a CTA runs its tiles in series, so a grid short of
+ * the SMs leaves them idle */
+static int wb_tiles_per_cta(size_t nsamp, int T, int nstreams, int nctile)
+{
+	int dev = 0, nsm = 132;
+	if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+	const size_t tiles = (nsamp + T - 1) / T * (size_t)nstreams * nctile;
+	return (int)std::max<size_t>(1, std::min<size_t>(8, tiles / ((size_t)8 * nsm)));
+}
+
 template <int KIND, bool OVL, int RB>
 static int launch_wb_t(const uint8_t *in, size_t stream_stride, const Hist &h, const float *p, const float2 *E, const int *meta,
                        float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
@@ -1595,13 +1606,7 @@ static int launch_wb_t(const uint8_t *in, size_t stream_stride, const Hist &h, c
 	if (e != cudaSuccess) return (int)e;
 	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 	if (e != cudaSuccess) return (int)e;
-	/* tiles per CTA: up to 8 (E is staged once per CTA), fewer where that would leave less than four waves of two CTAs
-	 * per SM — a CTA runs its tiles in series, so a grid short of the SMs leaves them idle */
-	int dev = 0, nsm = 132;
-	if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-	const size_t tiles = (nsamp + T - 1) / T * (size_t)nstreams * nctile;
-	const int tpc = (int)std::max<size_t>(1, std::min<size_t>(8, tiles / ((size_t)8 * nsm)));
-	const int rows_per_cta = tpc * T;
+	const int rows_per_cta = wb_tiles_per_cta(nsamp, T, nstreams, nctile) * T;
 	dim3 grid((unsigned)((nsamp + rows_per_cta - 1) / rows_per_cta), nstreams, nctile);
 	kern<<<grid, WB_THREADS, smem, stream>>>(in, stream_stride, reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad, h.pos0,
 	                                         p, E, meta, dm, K, nch, nctile, nsamp, rows_per_cta);
@@ -2141,6 +2146,229 @@ int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, c
 	if (K == 800) return ACB_ORD_GO(100, 8, 4);
 #undef ACB_ORD_GO
 	return (int)cudaErrorInvalidValue;
+}
+
+/* ------------------------------------------------------------------------------------------
+ * K1, wideband fast form for REAL input (ACB_FLAG_FAST_WIDEBAND_REAL; DESIGN.md §4): k_channelize_rdft's definition at
+ * taps = K (orc_channelize_rdft) and k_channelize_ovl_rdft's at taps > K (orc_ovl_presum_real, then orc_channelize_rdft)
+ * for any K % 8 == 0 up to ACB_MAXK and any channel count.  The narrow kernels put 8 channels in a CTA and redo the row's
+ * quarter split (and at taps > K the whole pre-sum) for every group of 8; here, as in k_channelize_wb, one CTA takes
+ * rows_per_cta rows (tiles of T rows) of one stream and up to WB_CTILE channels:
+ *
+ *   front half (once per row for all channels): at taps > K the pre-sum z_m[n] = sum_r p[n + H + r*K] * x[m*K + n + r*K]
+ *     in ascending tap order, one fmaf per term; then the quarter split per n2 < K/4: s02, s13, y0 = s02 + s13,
+ *     y2 = s02 - s13, d02, d13, the rounded additions orc_channelize_rdft makes for every channel, made once.  Into shared
+ *     memory as three columns [row][n2]: y0, y2 and (d02, d13), 4*K bytes per row.  Terms before the stream start READ
+ *     the history in front of the rows in d_real, which acb_create / acb_reset zero: as in k_channelize_ovl_rdft, z starts
+ *     at +0, those terms and the zero front padding of p come first, and fma(p, +-0, +0) = +0 leaves it there, so the sum
+ *     is that of the valid terms only.  Every fetch lies in [-hpad, nsamp*K) samples of the stream.
+ *   back half: a work item is WBR_RB rows x WB_CB channel slots of one column (k mod 4 = 0: y0; 2: y2; odd: d02 and d13
+ *     with two sums, residues 1 and 3 differing in one sign at the end).  LPR consecutive lanes share an item, lane h
+ *     summing the h-th range of ceil(K/8 / LPR) n2 pairs in n2 order; the LPR partial sums are then added by xor shuffles
+ *     in the definition's pairwise tree (h ^ 1, then h ^ 2, ...): k_channelize_rdft's ranges and tree, LPR = 2 / 4 / 8 for
+ *     K < 400 / < 800 / >= 800 (channelize_rdft_lanes_per_row), at any K.  The twiddles come from ONE table staged in
+ *     shared memory, E[r] = acb_fast_plan_air's T for (k*n2) % K = r in [0, K) (acb_wb_twiddles' real variant).  The
+ *     item's outputs are spread over its LPR lanes, which all hold the same sums.  |D| in double (envelope()): float
+ *     input has no bound.
+ *
+ * meta per (stream, channel tile) as k_channelize_wb's; the slots are sorted by column (context.cu: upload_wb_plan).
+ * ---------------------------------------------------------------------------------------- */
+constexpr int WBR_THREADS = 256;
+constexpr int WBR_RB = 4;                     /* rows per back-half item */
+
+template <int LPR, bool OVL>
+__global__ void __launch_bounds__(WBR_THREADS, 2)
+k_channelize_wb_real(const uint8_t *__restrict__ in, size_t stream_stride, int hpad, const float *__restrict__ pw,
+                     const float2 *__restrict__ E, const int *__restrict__ meta, float *__restrict__ dm, int K, int nch,
+                     int nctile, size_t nsamp, int T, int rows_per_cta)
+{
+	constexpr int RB = WBR_RB, CB = WB_CB;
+	const int N2 = K >> 2, K8 = K >> 3, PER = (K8 + LPR - 1) / LPR;
+	extern __shared__ __align__(16) unsigned char smem[];
+	float *Y0 = reinterpret_cast<float *>(smem);                         /* [row][n2] */
+	float *Y2 = Y0 + (size_t)T * N2;
+	float2 *DD = reinterpret_cast<float2 *>(Y2 + (size_t)T * N2);        /* (d02, d13) */
+	float2 *Es = DD + (size_t)T * N2;                                     /* E[r], r in [0, K) */
+	const int s = blockIdx.y;
+	const int *ms = meta + ((size_t)s * nctile + blockIdx.z) * WB_META;
+	const int ng = ms[0];
+	for (int i = threadIdx.x; i < K; i += WBR_THREADS) Es[i] = E[K - 1 + i];
+	const int nitem = (T / RB) * ng;
+
+	for (int t0 = 0; t0 < rows_per_cta; t0 += T) {
+		const size_t r0 = (size_t)blockIdx.x * rows_per_cta + t0;
+		if (r0 >= nsamp) break;
+		__syncthreads();                          /* E staged / the previous tile's Y' consumed */
+		const float *src = reinterpret_cast<const float *>(in + (size_t)s * stream_stride);   /* sample 0 of the submit */
+		for (int it = threadIdx.x; it < T * N2; it += WBR_THREADS) {
+			const int j = it / N2, n2 = it - j * N2;
+			const size_t row = r0 + j;
+			float y0 = 0.f, y2 = 0.f, d02 = 0.f, d13 = 0.f;
+			if (row < nsamp) {
+				float x[4];
+#pragma unroll
+				for (int q = 0; q < 4; q++) {
+					const int nn = q * N2 + n2;
+					const float *xs = src + (long long)row * K + nn;
+					if (!OVL) {
+						x[q] = __ldg(xs);
+					} else {
+						const int rlo = -((nn + hpad) / K);            /* >= -hpad samples: the history */
+						const float *pr = pw + nn + hpad;
+						float a = 0.f;
+						for (int r = rlo; r <= 0; r++) a = __fmaf_rn(__ldg(pr + r * K), __ldg(xs + (long long)r * K), a);
+						x[q] = a;
+					}
+				}
+				const float s02 = __fadd_rn(x[0], x[2]), s13 = __fadd_rn(x[1], x[3]);
+				y0 = __fadd_rn(s02, s13);
+				y2 = __fsub_rn(s02, s13);
+				d02 = __fsub_rn(x[0], x[2]);
+				d13 = __fsub_rn(x[1], x[3]);
+			}
+			Y0[it] = y0;
+			Y2[it] = y2;
+			DD[it] = make_float2(d02, d13);
+		}
+		__syncthreads();
+
+		/* items (row group, channel group), channel group fastest; a warp holds 32 / LPR whole items, so the shuffles
+		 * stay inside one; lanes past the last item run an empty range */
+		for (int u0 = 0; u0 < nitem * LPR; u0 += WBR_THREADS) {
+			const int u = u0 + (int)threadIdx.x, item = u / LPR, h = u & (LPR - 1);
+			const bool valid = item < nitem;
+			const int rg = valid ? item / ng : 0, cg = valid ? item - rg * ng : 0;
+			const int *sl = ms + 2 + 2 * cg * CB;
+			int kk[CB], idx[CB];
+			const int g0 = h * PER, g1 = valid ? min(K8, g0 + PER) : g0;
+#pragma unroll
+			for (int c = 0; c < CB; c++) {
+				kk[c] = sl[2 * c];
+				idx[c] = (kk[c] * 2 * g0) % K;        /* (k*n2) % K at the range's first n2, 0 <= k < K */
+			}
+			float acc[RB][CB][4];                     /* ax, ay, bx, by (orc_channelize_rdft) */
+#pragma unroll
+			for (int j = 0; j < RB; j++)
+#pragma unroll
+				for (int c = 0; c < CB; c++) acc[j][c][0] = acc[j][c][1] = acc[j][c][2] = acc[j][c][3] = 0.f;
+			const int col = kk[0] & 3;                /* slot 0 of a group is always a channel */
+			const int roff = rg * RB * N2;
+			if (col & 1) {
+				const float2 *Yr = DD + roff;
+#pragma unroll 1
+				for (int n2 = 2 * g0; n2 < 2 * g1; n2++) {
+					float2 t[CB];
+#pragma unroll
+					for (int c = 0; c < CB; c++) {
+						t[c] = Es[idx[c]];
+						const int v = idx[c] + kk[c];
+						idx[c] = v >= K ? v - K : v;
+					}
+#pragma unroll
+					for (int j = 0; j < RB; j++) {
+						const float2 d = Yr[j * N2 + n2];
+#pragma unroll
+						for (int c = 0; c < CB; c++) {
+							acc[j][c][0] = __fmaf_rn(d.x, t[c].x, acc[j][c][0]);
+							acc[j][c][1] = __fmaf_rn(d.x, t[c].y, acc[j][c][1]);
+							acc[j][c][2] = __fmaf_rn(d.y, t[c].x, acc[j][c][2]);
+							acc[j][c][3] = __fmaf_rn(d.y, t[c].y, acc[j][c][3]);
+						}
+					}
+				}
+			} else {
+				const float *Yr = (col == 0 ? Y0 : Y2) + roff;
+#pragma unroll 1
+				for (int n2 = 2 * g0; n2 < 2 * g1; n2++) {
+					float2 t[CB];
+#pragma unroll
+					for (int c = 0; c < CB; c++) {
+						t[c] = Es[idx[c]];
+						const int v = idx[c] + kk[c];
+						idx[c] = v >= K ? v - K : v;
+					}
+#pragma unroll
+					for (int j = 0; j < RB; j++) {
+						const float y = Yr[j * N2 + n2];
+#pragma unroll
+						for (int c = 0; c < CB; c++) {
+							acc[j][c][0] = __fmaf_rn(y, t[c].x, acc[j][c][0]);
+							acc[j][c][1] = __fmaf_rn(y, t[c].y, acc[j][c][1]);
+						}
+					}
+				}
+			}
+			/* the LPR partial sums, pairwise: (p0 + p1) + (p2 + p3) ... — every lane of the item computes the same sum */
+#pragma unroll
+			for (int step = 1; step < LPR; step *= 2)
+#pragma unroll
+				for (int j = 0; j < RB; j++)
+#pragma unroll
+					for (int c = 0; c < CB; c++)
+#pragma unroll
+						for (int q = 0; q < 4; q++)
+							acc[j][c][q] = __fadd_rn(acc[j][c][q], __shfl_xor_sync(0xffffffffu, acc[j][c][q], step));
+			if (!valid) continue;
+#pragma unroll
+			for (int j = 0; j < RB; j++) {
+				const size_t row = r0 + rg * RB + j;
+#pragma unroll
+				for (int c = 0; c < CB; c++) {
+					if (((j * CB + c) & (LPR - 1)) != h) continue;
+					const int chc = sl[2 * c + 1];
+					if (row >= nsamp || chc < 0) continue;
+					/* r = 1: D = (ax + by) + j (ay - bx); r = 3: the other signs; r even: b is zero */
+					const float sg = (kk[c] & 3) == 3 ? -1.0f : 1.0f;
+					const float re = __fadd_rn(acc[j][c][0], __fmul_rn(sg, acc[j][c][3]));
+					const float im = __fadd_rn(acc[j][c][1], -__fmul_rn(sg, acc[j][c][2]));
+					dm[((size_t)s * nsamp + row) * nch + chc] = envelope(make_float2(re, im));
+				}
+			}
+		}
+	}
+}
+
+/* rows per tile of k_channelize_wb_real: the most, a multiple of WBR_RB and at most 32, whose Y' (4*K bytes per row) and
+ * E (8*K bytes) leave room for two CTAs per SM (113 KB each): 32 rows up to K = 848, 12 at K = 2048; the most shared
+ * memory is 115 648 bytes (K = 1112, 24 rows) */
+static int wbr_rows(int K)
+{
+	return std::min(32, (113 * 1024 - 8 * K) / (4 * K) / WBR_RB * WBR_RB);
+}
+
+template <int LPR, bool OVL>
+static int launch_wbr_t(const uint8_t *in, size_t stream_stride, int hpad, const float *p, const float2 *E, const int *meta,
+                        float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	const int T = wbr_rows(K);
+	const int smem = 4 * T * K + 8 * K;
+	const int nctile = (nch + WB_CTILE - 1) / WB_CTILE;
+	auto kern = k_channelize_wb_real<LPR, OVL>;
+	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	if (e != cudaSuccess) return (int)e;
+	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	if (e != cudaSuccess) return (int)e;
+	const int rows_per_cta = wb_tiles_per_cta(nsamp, T, nstreams, nctile) * T;
+	dim3 grid((unsigned)((nsamp + rows_per_cta - 1) / rows_per_cta), nstreams, nctile);
+	kern<<<grid, WBR_THREADS, smem, stream>>>(in, stream_stride, hpad, p, E, meta, dm, K, nch, nctile, nsamp, T, rows_per_cta);
+	return (int)cudaGetLastError();
+}
+
+/* float32 real input, K % 8 == 0, K <= ACB_MAXK, any nch, every channel on the 12.5 kHz raster; taps = K (hpad = 0) or
+ * taps > K (`p` = taps_pad floats, fl(K*h) behind hpad - H zeros); `in` = sample 0 of stream 0's submit with each
+ * stream's hpad-sample history right in front of it (d_real); `nsamp` output rows per stream, any count */
+int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
+                              float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+{
+	if (nsamp == 0) return 0;
+	if ((K & 7) || K > 2048 || hpad < 0) return (int)cudaErrorInvalidValue;
+	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
+	const float2 *E2 = reinterpret_cast<const float2 *>(E);
+	const int lpr = channelize_rdft_lanes_per_row(K);
+#define ACB_WBR_GO(L, O) launch_wbr_t<L, O>(i8, stream_stride, hpad, p, E2, meta, dm, K, nch, nstreams, nsamp, stream)
+	if (hpad) return lpr == 8 ? ACB_WBR_GO(8, true) : lpr == 4 ? ACB_WBR_GO(4, true) : ACB_WBR_GO(2, true);
+	return lpr == 8 ? ACB_WBR_GO(8, false) : lpr == 4 ? ACB_WBR_GO(4, false) : ACB_WBR_GO(2, false);
+#undef ACB_WBR_GO
 }
 
 bool channelize_dft_supports(int K) { return K == 160 || K == 192; }

@@ -126,7 +126,24 @@ typedef struct {
                                          with the same tolerances.  Where ACB_FLAG_FAST_CHANNELIZER or ACB_FLAG_FAST_FILTER
                                          also applies (K = 160 or 192) their kernels run; the bits are the same.  Anything
                                          else runs what runs without this flag: taps < K, acb_set_wf tables, a stream off the
-                                         raster, K % 8 != 0, real input (no effect).  ACB_FAST_FOLD8 does not apply. */
+                                         raster, K % 8 != 0, real input (no effect; real input has its own bit,
+                                         ACB_FLAG_FAST_WIDEBAND_REAL).  ACB_FAST_FOLD8 does not apply. */
+#define ACB_FLAG_FAST_WIDEBAND_REAL 128 /* real-input contexts (ACB_FLAG_REAL_INPUT) with K % 8 == 0 (K <= ACB_MAXK), any nch,
+                                         taps >= K, every stream planned by acb_set_plan_air with acb_fast_plan_air returning
+                                         1 (every channel on the 12.5 kHz raster): the real-input fast forms for any shape.
+                                         The row's shared work (the quarter split, and at taps > K the pre-sum) is done once
+                                         per row for all channels, and every channel's twiddles come from one table per
+                                         context.  At taps = K the envelope is bit-identical to ACB_FLAG_FAST_CHANNELIZER's
+                                         real-input definition (oracle orc_channelize_rdft, its lanes-per-row ranges and
+                                         pairwise tree included, at any such K), at taps > K to ACB_FLAG_FAST_FILTER_REAL's
+                                         (the pre-sum, then the same), with the same tolerances: per output row, with
+                                         S = sum |x|*|w|, within 1e-5*S of the exact form's envelope and within 1e-6*S of the
+                                         float64 definition; decoded messages are the same.  Where ACB_FLAG_FAST_CHANNELIZER
+                                         (taps = K) or ACB_FLAG_FAST_FILTER_REAL (taps > K) also applies (K = 200, 240, 400,
+                                         480 or 800) their kernels run; the bits are the same.  Anything else runs what runs
+                                         without this flag: taps < K, acb_set_wf tables, a stream off the raster,
+                                         K % 8 != 0; on u8 and CS16 contexts this flag has no effect, and
+                                         ACB_FLAG_FAST_WIDEBAND alone selects nothing on a real context. */
 #define ACB_FLAG_REAL_INPUT 2         /* Airspy front-end (air.c): float32 REAL samples at IF = rate/4,
                                          rate = K*12500; use acb_set_plan_air / acb_submit_real_host */
 
@@ -377,7 +394,7 @@ typedef struct {
 	uint64_t chan_launches, demod_launches;
 	uint64_t fast_chan_launches; /* channelizer launches that took a fast form: ACB_FLAG_FAST_CHANNELIZER's (taps = K) or
 	                                ACB_FLAG_FAST_FILTER's or ACB_FLAG_FAST_FILTER_REAL's (taps > K),
-	                                or ACB_FLAG_FAST_WIDEBAND's (either) */
+	                                or ACB_FLAG_FAST_WIDEBAND's or ACB_FLAG_FAST_WIDEBAND_REAL's (either) */
 	uint64_t frames_lost;       /* frames that found the device ring full (ACB_ERR_OVERFLOW was returned once per submit) */
 	double   host_ms;           /* accumulated wall time the consumer thread spent ordering and queuing frames */
 } acb_stats_t;

@@ -73,4 +73,15 @@ with api.Context(Kw, 1, 13, 1, flags=4 | api.FLAG_FAST_WIDEBAND, taps=2 * Kw + 3
         ctx.submit_cs16(part)
     ctx.sync()
     assert ctx.stats().fast_chan_launches == 2          # the 1000-sample submit completes no row
+# the real-input wideband fast form at its largest shared-memory configuration (K = 1112: 24-row tiles, 115648 bytes per
+# CTA), taps > K (the history in front of the rows), ragged real submits, every residue k mod 4
+Kr = 1112
+fr = [131_500_000 + 12_500 * d for d in (-200, -151, -150, -149, -100, -3, -2, -1, 0, 1, 50, 101, 150)]
+xr = (np.random.default_rng(2).standard_normal((1, 40 * Kr + 77)) * 100).astype(np.float32)
+with api.Context(Kr, 1, 13, 1, flags=2 | api.FLAG_FAST_WIDEBAND_REAL, taps=2 * Kr + 3) as ctx:
+    ctx.set_plan_air(0, fr)
+    for part in (xr, xr[:, :1000], xr[:, :17 * Kr + 3]):
+        ctx.submit_real(part)
+    ctx.sync()
+    assert ctx.stats().fast_chan_launches == 2          # the 1000-sample submit completes no row
 print("sanitize run ok", n1, n3, n4, n5)
