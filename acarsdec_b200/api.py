@@ -111,6 +111,7 @@ ABI = [
     ("acb_version", C.c_char_p, []),
     ("acb_set_plan", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_uint)]),
     ("acb_set_plan_air", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_uint)]),
+    ("acb_set_plan_air_at", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_uint]),
     ("acb_set_plan_cs16", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_uint, C.POINTER(C.c_uint)]),
     ("acb_set_plan_at", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_uint]),
     ("acb_set_wf", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
@@ -133,6 +134,12 @@ ABI = [
     ("acb_multi_set_wf", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     ("acb_multi_reset", C.c_int, [C.c_void_p]),
     ("acb_multi_submit_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_multi_set_plan_air", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_uint)]),
+    ("acb_multi_set_plan_cs16", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_uint, C.POINTER(C.c_uint)]),
+    ("acb_multi_submit_real_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_multi_submit_cs16_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_multi_submit_cs16_planar_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_multi_set_emission_groups", C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
     ("acb_multi_collect", C.c_int, [C.c_void_p]),
     ("acb_multi_sync", C.c_int, [C.c_void_p]),
     ("acb_multi_drain", C.c_int, [C.c_void_p, C.POINTER(Msg), C.c_int]),
@@ -450,6 +457,11 @@ class Context:
         _check(self.lib, self.lib.acb_set_plan_air(self.h, stream, f.ctypes.data, len(f), C.byref(fc)))
         return fc.value
 
+    def set_plan_air_at(self, stream: int, freqs_hz, fc_hz: int) -> None:
+        """set_plan_air around a given tuner centre (a context serving some of a receiver's channels)."""
+        f = np.asarray(freqs_hz, dtype=np.uint32)
+        _check(self.lib, self.lib.acb_set_plan_air_at(self.h, stream, f.ctypes.data, len(f), int(fc_hz)))
+
     @staticmethod
     def _stream_stride(a: np.ndarray, sample_bytes: int, stream_stride: int | None) -> int:
         """Stream stride in samples: the array's row pitch (a view into wider rows keeps its pitch), which an explicit
@@ -644,6 +656,49 @@ class MultiContext:
         assert iq.dtype == np.uint8 and iq.flags.c_contiguous
         stride = iq.strides[0] if iq.ndim == 2 else nblk * OUTBLK * self.K * 2
         _check(self.lib, self.lib.acb_multi_submit_host(self.h, iq.ctypes.data, stride, nblk))
+
+    def set_plan_air(self, stream: int, freqs_hz) -> int:
+        """Real input: Fc chosen once over all channels (acb_air_choose_fc), every part planned around it."""
+        f = np.asarray(freqs_hz, dtype=np.uint32)
+        fc = C.c_uint()
+        _check(self.lib, self.lib.acb_multi_set_plan_air(self.h, stream, f.ctypes.data, len(f), C.byref(fc)))
+        return fc.value
+
+    def set_plan_cs16(self, stream: int, freqs_hz, variant: int, fc_hz: int = 0) -> int:
+        f = np.asarray(freqs_hz, dtype=np.uint32)
+        fc = C.c_uint()
+        _check(self.lib, self.lib.acb_multi_set_plan_cs16(self.h, stream, f.ctypes.data, len(f), variant, fc_hz, C.byref(fc)))
+        return fc.value
+
+    # the streaming submits take what Context's take, with the same stride rules
+    def submit_real(self, x: np.ndarray, stream_stride: int | None = None) -> int:
+        assert x.dtype == np.float32 and x.ndim == 2 and x.shape[0] == self.nstreams
+        stride = Context._stream_stride(x, 4, stream_stride)
+        return _check(self.lib, self.lib.acb_multi_submit_real_host(self.h, x.ctypes.data, stride, x.shape[1]))
+
+    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None) -> int:
+        assert iq.dtype == np.int16 and iq.ndim == 3 and iq.shape[0] == self.nstreams and iq.shape[2] == 2 and iq.strides[2] == 2
+        stride = Context._stream_stride(iq, 4, stream_stride)
+        return _check(self.lib, self.lib.acb_multi_submit_cs16_host(self.h, iq.ctypes.data, stride, iq.shape[1]))
+
+    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None) -> int:
+        assert xi.dtype == np.int16 and xq.dtype == np.int16 and xi.shape == xq.shape and xi.shape[0] == self.nstreams
+        stride = Context._stream_stride(xi, 2, stream_stride)
+        assert Context._stream_stride(xq, 2, stream_stride) == stride
+        return _check(self.lib, self.lib.acb_multi_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, stride, xi.shape[1]))
+
+    def set_emission_groups(self, unit: int, period: int = 0) -> None:
+        """As Context.set_emission_groups; the merged order follows these groups."""
+        _check(self.lib, self.lib.acb_multi_set_emission_groups(self.h, unit, period))
+
+    def reset(self) -> None:
+        _check(self.lib, self.lib.acb_multi_reset(self.h))
+
+    def part_stats(self, i: int, reset: bool = False) -> Stats:
+        """acb_get_stats of the i-th per-device context."""
+        s = Stats()
+        _check(self.lib, self.lib.acb_get_stats(self.lib.acb_multi_part(self.h, i), C.byref(s), int(reset)))
+        return s
 
     def sync(self) -> int:
         return _check(self.lib, self.lib.acb_multi_sync(self.h))

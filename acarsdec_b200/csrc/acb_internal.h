@@ -2,7 +2,10 @@
 #ifndef ACB_INTERNAL_H
 #define ACB_INTERNAL_H
 
+#include <stddef.h>
 #include <stdint.h>
+
+#include <vector>
 
 namespace acb {
 
@@ -115,6 +118,13 @@ int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_st
                            size_t nsamples, int nstreams, CUstream_st *stream);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
+
+/* context.cu, host side, shared with multi.cpp */
+/* sets the message acb_last_error() returns (of the calling thread); returns `code` */
+int fail(int code, const char *fmt, ...);
+/* Emission-group starts of a streaming submit that covers envelope samples [pos, pos + nout): the first is pos, then
+ * one per `period` outputs (ACB_GROUP_OUTPUTS) or per transfer of `period` input samples (ACB_GROUP_INPUT) */
+std::vector<unsigned long long> stream_groups(int unit, unsigned long long period, int K, unsigned long long pos, size_t nout);
 } // namespace acb
 
 #endif

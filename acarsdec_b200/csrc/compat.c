@@ -125,15 +125,50 @@ static void deliver(const acb_msg_t *m, int chn, const struct timeval *tv)
 }
 
 /* everything the library has queued -> the consumer, stamped with the time of its SOH sample */
-static void deliver_ready(acb_ctx_t *ctx) __attribute__((unused));
-static void deliver_ready(acb_ctx_t *ctx)
+static void deliver_ready(acb_multi_t *m) __attribute__((unused));
+static void deliver_ready(acb_multi_t *m)
 {
 	acb_msg_t out[16];
-	for (int n; (n = acb_drain(ctx, out, 16)) > 0;)
+	for (int n; (n = acb_multi_drain(m, out, 16)) > 0;)
 		for (int i = 0; i < n; i++) {
 			const struct timeval tv = stamp_time(out[i].soh_pos);      /* acars.c:290 */
 			deliver(&out[i], out[i].chn, &tv);
 		}
+}
+
+/* The front-ends serve one stream with nbch channels: on one GPU, or with ACARSDEC_B200_DEVICES=0,1,... the channels
+ * split over several (acb_multi_*, channel-split mode): the unmodified C host reaches a whole node this way.  Without
+ * the list, ACARSDEC_B200_DEVICE names the one device (default 0). */
+static int parse_devices(int *dev, int max) __attribute__((unused));
+static int parse_devices(int *dev, int max)
+{
+	const char *e = getenv("ACARSDEC_B200_DEVICES");
+	int n = 0;
+	if (e && *e) {
+		char *dup = strdup(e), *save = NULL;
+		for (char *t = strtok_r(dup, ",", &save); t && n < max; t = strtok_r(NULL, ",", &save)) dev[n++] = atoi(t);
+		free(dup);
+	}
+	if (n == 0) {
+		e = getenv("ACARSDEC_B200_DEVICE");
+		dev[n++] = e ? atoi(e) : 0;
+	}
+	return n;
+}
+
+/* one stream, nbch channels, split over the devices parse_devices names */
+static acb_multi_t *front_end_create(acb_config_t *cfg) __attribute__((unused));
+static acb_multi_t *front_end_create(acb_config_t *cfg)
+{
+	int devs[MAXNBCHANNELS];
+	const int ndev = parse_devices(devs, MAXNBCHANNELS);
+	acb_multi_t *m = NULL;
+	if (acb_multi_create(cfg, devs, ndev, ACB_MULTI_SPLIT_CHANNELS, &m) != ACB_OK) {
+		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
+		if (m) acb_multi_destroy(m);
+		return NULL;
+	}
+	return m;
 }
 
 /* ---------------------------------------------------------------- initAcars / deinitAcars */
@@ -342,36 +377,9 @@ static int env_taps(int K, int *taps)
 
 #ifdef WITH_RTL
 
-/* One stream, nbch channels — on one GPU, or with ACARSDEC_B200_DEVICES=0,1,... the channels split over
- * several (acb_multi_*, channel-split mode): the unmodified C host reaches a whole node this way. */
 static acb_multi_t *rtl_ctx;
 static FILE *rtl_src;
 
-static int parse_devices(int *dev, int max)
-{
-	const char *e = getenv("ACARSDEC_B200_DEVICES");
-	int n = 0;
-	if (e && *e) {
-		char *dup = strdup(e), *save = NULL;
-		for (char *t = strtok_r(dup, ",", &save); t && n < max; t = strtok_r(NULL, ",", &save)) dev[n++] = atoi(t);
-		free(dup);
-	}
-	if (n == 0) {
-		e = getenv("ACARSDEC_B200_DEVICE");
-		dev[n++] = e ? atoi(e) : 0;
-	}
-	return n;
-}
-
-static void rtl_deliver_ready(void)
-{
-	acb_msg_t out[16];
-	for (int n; (n = acb_multi_drain(rtl_ctx, out, 16)) > 0;)
-		for (int i = 0; i < n; i++) {
-			const struct timeval tv = stamp_time(out[i].soh_pos);      /* acars.c:290 */
-			deliver(&out[i], out[i].chn, &tv);
-		}
-}
 static int rtl_batch = 16;              /* blocks per submit; ACARSDEC_B200_BLOCKS */
 static volatile int rtl_cancel;
 static size_t rtl_inbufsize;
@@ -420,14 +428,7 @@ int initRtl(char **argv, int optind)
 	if (e && atoi(e) > 0) rtl_batch = atoi(e);
 	acb_config_t cfg = { 0, rtlMult, 1, (int)nbch, rtl_batch, 0, 0 };
 	if (env_taps(rtlMult, &cfg.taps)) return 1;
-	int devs[MAXNBCHANNELS];
-	const int ndev = parse_devices(devs, MAXNBCHANNELS);
-	if (acb_multi_create(&cfg, devs, ndev, ACB_MULTI_SPLIT_CHANNELS, &rtl_ctx) != ACB_OK) {
-		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
-		if (rtl_ctx) acb_multi_destroy(rtl_ctx);
-		rtl_ctx = NULL;
-		return 1;
-	}
+	if (!(rtl_ctx = front_end_create(&cfg))) return 1;
 	float *wf = malloc(sizeof(float) * 2 * rtlMult * nbch);
 	if (!wf) return 1;
 	for (unsigned n = 0; n < nbch; n++) {                        /* rtl.c:272-287 */
@@ -477,7 +478,7 @@ int runRtlSample(void)
 			rc = acb_multi_collect(rtl_ctx);
 			if (rc < 0) break;
 			inflight--;
-			rtl_deliver_ready();
+			deliver_ready(rtl_ctx);
 		}
 		size_t got = fread(buf[which], 1, rtl_inbufsize * rtl_batch, rtl_src);
 		int nblk = (int)(got / rtl_inbufsize);
@@ -493,7 +494,7 @@ int runRtlSample(void)
 	}
 	if (rc >= 0) rc = acb_multi_sync(rtl_ctx);
 	if (rc < 0) fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
-	rtl_deliver_ready();
+	deliver_ready(rtl_ctx);
 	for (unsigned n = 0; n < nbch; n++)
 		if (acb_multi_get_state(rtl_ctx, 0, (int)n, &st) == ACB_OK) state_unpack(&st, &channel[n]);
 	for (int i = 0; i < 2; i++) acb_host_free(buf[i]);
@@ -521,7 +522,7 @@ int runRtlClose(void)
 
 #ifdef WITH_AIR
 
-static acb_ctx_t *air_ctx;
+static acb_multi_t *air_ctx;
 static FILE *air_src;
 static unsigned air_rate, air_mult;
 static volatile int air_cancel;
@@ -567,13 +568,7 @@ int initAirspy(char **argv, int optind)
 	const int maxblk = (AIR_TRANSFER * 8 / (int)air_mult) / RTLOUTBUFSZ + 2;
 	acb_config_t cfg = { 0, (int)air_mult, 1, (int)nbch, maxblk, ACB_FLAG_REAL_INPUT, 0 };
 	if (env_taps((int)air_mult, &cfg.taps)) return -1;
-	if ((e = getenv("ACARSDEC_B200_DEVICE"))) cfg.device = atoi(e);
-	if (acb_create(&cfg, &air_ctx) != ACB_OK) {
-		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
-		if (air_ctx) acb_destroy(air_ctx);
-		air_ctx = NULL;
-		return -1;
-	}
+	if (!(air_ctx = front_end_create(&cfg))) return -1;
 	float *wf = malloc(sizeof(float) * 2 * air_mult * nbch);
 	if (!wf) return -1;
 	for (unsigned n = 0; n < nbch; n++) {                                 /* air.c:263-285 */
@@ -586,7 +581,7 @@ int initAirspy(char **argv, int optind)
 		for (unsigned i = 0; i < air_mult; i++)
 			ch->wf[i] = wf[((size_t)n * air_mult + i) * 2] + wf[((size_t)n * air_mult + i) * 2 + 1] * I;
 	}
-	int rc = cfg.taps ? acb_set_plan_air(air_ctx, 0, Fd, (int)nbch, NULL) : acb_set_wf(air_ctx, 0, wf, (int)nbch);
+	int rc = cfg.taps ? acb_multi_set_plan_air(air_ctx, 0, Fd, (int)nbch, NULL) : acb_multi_set_wf(air_ctx, 0, wf, (int)nbch);
 	free(wf);
 	if (rc != ACB_OK) { fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error()); return -1; }
 	return 0;
@@ -603,36 +598,36 @@ int runAirspySample(void)
 	float *buf[2] = { acb_host_alloc(cap * sizeof(float)), acb_host_alloc(cap * sizeof(float)) };
 	if (!buf[0] || !buf[1]) { fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error()); return -1; }
 	acb_chan_state_t st;
-	for (unsigned n = 0; n < nbch; n++) { state_pack(&channel[n], &st); acb_set_state(air_ctx, 0, (int)n, &st); }
-	acb_set_emission_groups(air_ctx, ACB_GROUP_INPUT, AIR_TRANSFER);
+	for (unsigned n = 0; n < nbch; n++) { state_pack(&channel[n], &st); acb_multi_set_state(air_ctx, 0, (int)n, &st); }
+	acb_multi_set_emission_groups(air_ctx, ACB_GROUP_INPUT, AIR_TRANSFER);
 	int rc = ACB_OK, which = 0, inflight = 0;
 	uint64_t pos = 0;
 	stamp_reset();
 	while (!signalExit && !air_cancel) {
 		if (inflight == 2) {                 /* buf[which] fed the submit two back: it has been consumed */
-			rc = acb_collect(air_ctx);
+			rc = acb_multi_collect(air_ctx);
 			if (rc < 0) break;
 			inflight--;
 			deliver_ready(air_ctx);
 		}
 		size_t got = fread(buf[which], sizeof(float), cap, air_src);
 		if (got == 0) break;
-		rc = acb_submit_real_host(air_ctx, buf[which], got, got);
+		rc = acb_multi_submit_real_host(air_ctx, buf[which], got, got);
 		if (rc < 0) break;
 		if (rc > 0) { pos += (uint64_t)rc; inflight++; which ^= 1; }
-		else if ((rc = acb_sync(air_ctx)) < 0) break;             /* fewer samples than one output row: copy done before reuse */
+		else if ((rc = acb_multi_sync(air_ctx)) < 0) break;             /* fewer samples than one output row: copy done before reuse */
 		else inflight = 0;
 		stamp_batch(pos);
 		if (got < cap) break;
 	}
-	if (rc >= 0) rc = acb_sync(air_ctx);
+	if (rc >= 0) rc = acb_multi_sync(air_ctx);
 	if (rc < 0) fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
 	deliver_ready(air_ctx);
 	for (unsigned n = 0; n < nbch; n++)
-		if (acb_get_state(air_ctx, 0, (int)n, &st) == ACB_OK) state_unpack(&st, &channel[n]);
+		if (acb_multi_get_state(air_ctx, 0, (int)n, &st) == ACB_OK) state_unpack(&st, &channel[n]);
 	acb_host_free(buf[0]);
 	acb_host_free(buf[1]);
-	acb_destroy(air_ctx);
+	acb_multi_destroy(air_ctx);
 	air_ctx = NULL;
 	return rc < 0 ? -1 : 0;
 }
@@ -643,7 +638,7 @@ int runAirspySample(void)
 
 #if defined(WITH_SOAPY) || defined(WITH_SDRPLAY)
 
-static acb_ctx_t *cs_ctx;
+static acb_multi_t *cs_ctx;
 static FILE *cs_src;
 static int cs_mult;
 #define CS_BATCH 8                  /* blocks of 1024*mult complex samples per submit */
@@ -671,16 +666,9 @@ static int cs16_setup(const char *path, char **argv, int optind, int mult, int v
 	if (nbch == 0) { fprintf(stderr, "Need a least one frequency\n"); return 1; }
 	acb_config_t cfg = { 0, mult, 1, (int)nbch, CS_BATCH, ACB_FLAG_CS16_INPUT, 0 };
 	if (env_taps(mult, &cfg.taps)) return -1;
-	const char *e = getenv("ACARSDEC_B200_DEVICE");
-	if (e) cfg.device = atoi(e);
-	if (acb_create(&cfg, &cs_ctx) != ACB_OK) {
-		fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
-		if (cs_ctx) acb_destroy(cs_ctx);
-		cs_ctx = NULL;
-		return -1;
-	}
+	if (!(cs_ctx = front_end_create(&cfg))) return -1;
 	unsigned Fc = 0;
-	if (acb_set_plan_cs16(cs_ctx, 0, Fd, (int)nbch, variant, fc_user, &Fc) != ACB_OK) {
+	if (acb_multi_set_plan_cs16(cs_ctx, 0, Fd, (int)nbch, variant, fc_user, &Fc) != ACB_OK) {
 		fprintf(stderr, "%s\n", acb_last_error());            /* "Frequencies too far apart" */
 		return 1;
 	}
@@ -710,35 +698,35 @@ static int cs16_run(int group_outputs)
 	int16_t *buf[2] = { acb_host_alloc(cap * 2 * sizeof(int16_t)), acb_host_alloc(cap * 2 * sizeof(int16_t)) };
 	if (!buf[0] || !buf[1]) { fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error()); return -1; }
 	acb_chan_state_t st;
-	for (unsigned n = 0; n < nbch; n++) { state_pack(&channel[n], &st); acb_set_state(cs_ctx, 0, (int)n, &st); }
+	for (unsigned n = 0; n < nbch; n++) { state_pack(&channel[n], &st); acb_multi_set_state(cs_ctx, 0, (int)n, &st); }
 	/* the reference runs demodMSK channel by channel whenever dm_buffer is full (soapy.c:247: 1024 outputs,
 	 * sdrplay.c:229: 512): frames are queued in that order */
-	acb_set_emission_groups(cs_ctx, ACB_GROUP_OUTPUTS, (uint64_t)group_outputs);
+	acb_multi_set_emission_groups(cs_ctx, ACB_GROUP_OUTPUTS, (uint64_t)group_outputs);
 	int rc = ACB_OK, which = 0, inflight = 0;
 	uint64_t pos = 0;
 	stamp_reset();
 	while (!signalExit) {
 		if (inflight == 2) {                 /* buf[which] fed the submit two back: it has been consumed */
-			rc = acb_collect(cs_ctx);
+			rc = acb_multi_collect(cs_ctx);
 			if (rc < 0) break;
 			inflight--;
 			deliver_ready(cs_ctx);
 		}
 		size_t got = fread(buf[which], 2 * sizeof(int16_t), cap, cs_src);
 		if (got == 0) break;
-		rc = acb_submit_cs16_host(cs_ctx, buf[which], got, got);      /* any count: the remainder is carried */
+		rc = acb_multi_submit_cs16_host(cs_ctx, buf[which], got, got);      /* any count: the remainder is carried */
 		if (rc < 0) break;
 		if (rc > 0) { pos += (uint64_t)rc; inflight++; which ^= 1; }
-		else if ((rc = acb_sync(cs_ctx)) < 0) break;
+		else if ((rc = acb_multi_sync(cs_ctx)) < 0) break;
 		else inflight = 0;
 		stamp_batch(pos);
 		if (got < cap) break;
 	}
-	if (rc >= 0) rc = acb_sync(cs_ctx);
+	if (rc >= 0) rc = acb_multi_sync(cs_ctx);
 	if (rc < 0) fprintf(stderr, "acarsdec_b200: %s\n", acb_last_error());
 	deliver_ready(cs_ctx);
 	for (unsigned n = 0; n < nbch; n++)
-		if (acb_get_state(cs_ctx, 0, (int)n, &st) == ACB_OK) state_unpack(&st, &channel[n]);
+		if (acb_multi_get_state(cs_ctx, 0, (int)n, &st) == ACB_OK) state_unpack(&st, &channel[n]);
 	acb_host_free(buf[0]);
 	acb_host_free(buf[1]);
 	signalExit = 1;
@@ -747,7 +735,7 @@ static int cs16_run(int group_outputs)
 
 static void cs16_close(void)
 {
-	if (cs_ctx) { acb_destroy(cs_ctx); cs_ctx = NULL; }
+	if (cs_ctx) { acb_multi_destroy(cs_ctx); cs_ctx = NULL; }
 	if (cs_src && cs_src != stdin) fclose(cs_src);
 	cs_src = NULL;
 }

@@ -44,7 +44,7 @@ extern "C" void acb_build_sincos_table(double *cos_hi_lo, double *sin_hi_lo);
 
 static thread_local char g_err[512] = "";
 
-static int fail(int code, const char *fmt, ...)
+int acb::fail(int code, const char *fmt, ...)
 {
 	va_list ap;
 	va_start(ap, fmt);
@@ -1035,15 +1035,16 @@ extern "C" int acb_set_emission_groups(acb_ctx_t *c, int unit, uint64_t period)
 /* Emission groups of one streaming submit covering envelope samples [pos, pos + nout): the reference hands a
  * channel's new samples to demodMSK per transfer (air.c:336: output m completes with input sample (m+1)K - 1, so
  * transfer g of T samples starts at output floor(g*T/K)) or per full dm_buffer (soapy.c:247 every 1024 outputs,
- * sdrplay.c:229 every 512), channel by channel: frames leave in (group, channel, time) order. */
-static std::vector<unsigned long long> stream_groups(const acb_ctx *c, size_t nout)
+ * sdrplay.c:229 every 512), channel by channel: frames leave in (group, channel, time) order.  acb_multi_* keys its merge
+ * on the same starts. */
+std::vector<unsigned long long> acb::stream_groups(int unit, unsigned long long period, int Kc, unsigned long long pos, size_t nout)
 {
-	std::vector<unsigned long long> g{ c->pos };
-	const unsigned long long lo = c->pos, hi = c->pos + nout, K = (unsigned long long)c->cfg.K;
-	if (c->group_unit == ACB_GROUP_OUTPUTS) {
-		for (unsigned long long b = (lo / c->group_period + 1) * c->group_period; b < hi; b += c->group_period) g.push_back(b);
-	} else if (c->group_unit == ACB_GROUP_INPUT) {
-		const unsigned long long T = c->group_period;
+	std::vector<unsigned long long> g{ pos };
+	const unsigned long long lo = pos, hi = pos + nout, K = (unsigned long long)Kc;
+	if (unit == ACB_GROUP_OUTPUTS) {
+		for (unsigned long long b = (lo / period + 1) * period; b < hi; b += period) g.push_back(b);
+	} else if (unit == ACB_GROUP_INPUT) {
+		const unsigned long long T = period;
 		for (unsigned long long t = (lo * K) / T + 1;; t++) {        /* transfers that start after output `lo` began */
 			const unsigned long long b = t * T / K;                  /* first output completed inside transfer t */
 			if (b >= hi) break;
@@ -1094,7 +1095,8 @@ static int submit4(acb_ctx *c, const void *x, const void *x2, size_t stride_samp
 	CU(cudaStreamWaitEvent(c->s_comp, c->ev_real_copied, 0));
 	const size_t rem = total - nout * K;
 	if (nout) {
-		if (int r = run_kernels(c, (const uint8_t *)buf, c->real_cap * sizeof(float), 0, (int)nout, nullptr, stream_groups(c, nout)))
+		if (int r = run_kernels(c, (const uint8_t *)buf, c->real_cap * sizeof(float), 0, (int)nout, nullptr,
+		                        stream_groups(c->group_unit, c->group_period, c->cfg.K, c->pos, nout)))
 			return r;
 		c->pos += nout;
 		/* the unconsumed tail (air.c:329-334 / soapy.c:238-252 keep a partial sum instead: same
@@ -1159,22 +1161,24 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 	return upload_fast_plan(c, stream, ok, kbin, tw1);
 }
 
-extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
+static int check_plan_air(acb_ctx *c, const unsigned *freqs_hz, int nch)
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_F32REAL || nch != c->cfg.nch) return fail(ACB_ERR_ARG, "not a real-input context / nch mismatch");
 	if (c->taps < c->cfg.K) return fail(ACB_ERR_ARG, "taps < K: supply the tables with acb_set_wf");
-	unsigned lo = freqs_hz[0], hi = freqs_hz[0];
-	for (int i = 1; i < nch; i++) { lo = std::min(lo, freqs_hz[i]); hi = std::max(hi, freqs_hz[i]); }
+	return ACB_OK;
+}
+
+/* the tables and fast plans of a real-input stream around a given Fc (air.c:263-285) */
+static int plan_air(acb_ctx *c, int stream, const unsigned *freqs_hz, int nch, unsigned fc)
+{
 	const unsigned rate = (unsigned)c->cfg.K * ACB_INTRATE;
-	const unsigned fc = acb_air_choose_fc(lo, hi);
 	const int T = c->taps;
 	std::vector<float> wf((size_t)nch * T * 2);
 	for (int ch = 0; ch < nch; ch++) {
 		if (c->hpad) acb_air_build_wf_lp((int)freqs_hz[ch], (int)fc, rate, T, &wf[(size_t)ch * T * 2]);
 		else acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, &wf[(size_t)ch * T * 2]);
 	}
-	if (fc_out) *fc_out = fc;
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
 	std::vector<int> kbin(nch);
 	if (c->wb) return upload_wb_plan(c, stream, acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), nullptr) == 1, kbin, 0);
@@ -1182,6 +1186,23 @@ extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_
 	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
 	const bool ok = acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;
 	return upload_fast_plan(c, stream, ok, kbin, tw1);
+}
+
+extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
+{
+	if (int r = check_plan_air(c, freqs_hz, nch)) return r;
+	unsigned lo = freqs_hz[0], hi = freqs_hz[0];
+	for (int i = 1; i < nch; i++) { lo = std::min(lo, freqs_hz[i]); hi = std::max(hi, freqs_hz[i]); }
+	const unsigned fc = acb_air_choose_fc(lo, hi);
+	if (fc_out) *fc_out = fc;
+	return plan_air(c, stream, freqs_hz, nch, fc);
+}
+
+extern "C" int acb_set_plan_air_at(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned fc)
+{
+	if (int r = check_plan_air(c, freqs_hz, nch)) return r;
+	if (fc == 0) return fail(ACB_ERR_PLAN, "centre frequency 0");
+	return plan_air(c, stream, freqs_hz, nch, fc);
 }
 
 extern "C" int acb_submit_dm_host(acb_ctx_t *c, const float *dm, int nsamp)

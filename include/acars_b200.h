@@ -284,6 +284,10 @@ int acb_set_plan(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, 
 int acb_set_plan_at(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, unsigned fc_hz);
 /* The channel part of initAirspy (air.c:165-285) for a real-input context. */
 int acb_set_plan_air(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out);
+/* Same with the tuner centre given instead of acb_air_choose_fc's choice over these channels (a context that serves only
+ * SOME of a receiver's channels: acb_multi_set_plan_air in channel-split mode).  Tables and fast plans as acb_set_plan_air
+ * builds them; fc_hz = 0 is ACB_ERR_PLAN. */
+int acb_set_plan_air_at(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, unsigned fc_hz);
 /* The channel part of initSoapy (soapy.c:112-163) / initSdrplay (sdrplay.c:95-138) for a CS16
  * context; fc_hz = 0 lets chooseFc pick the centre (soapy.c:132-133 honours a user frequency). */
 int acb_set_plan_cs16(acb_ctx_t *ctx, int stream, const unsigned *freqs_hz, int nch, int variant, unsigned fc_hz, unsigned *fc_out);
@@ -407,11 +411,21 @@ int acb_get_stats(acb_ctx_t *ctx, acb_stats_t *out, int reset);
  *   ACB_MULTI_SPLIT_STREAMS   device d serves a contiguous range of the streams (BASELINE config 4);
  *   ACB_MULTI_SPLIT_CHANNELS  every device sees every stream and serves a contiguous range of its channels
  *                             (one wide stream, configs 3/5); each device fetches the block over its own PCIe link.
- * Stream / channel indices in the API and in the messages are global; messages are merged into the reference's
- * emission order (block, stream, channel, time; rtl.c:357-360).  cfg->device is ignored, `devices` names the
+ * Every input kind: u8 IQ (acb_multi_set_plan, acb_multi_submit_host), real input (cfg->flags ACB_FLAG_REAL_INPUT:
+ * acb_multi_set_plan_air, acb_multi_submit_real_host) and CS16 (ACB_FLAG_CS16_INPUT: acb_multi_set_plan_cs16,
+ * acb_multi_submit_cs16_host, acb_multi_submit_cs16_planar_host).  Each part is an ordinary context of cfg's kind and
+ * flags, so it runs the kernels (fast and wideband forms included) a single context would; a submit of the wrong kind
+ * is refused as the single-context call refuses it.  Arguments, return values and input lifetime are the single-context
+ * calls'; in a channel split every part reads the whole input, in a stream split part p reads from stream s0(p).  The
+ * planners choose the centre once over all channels of the stream and give it to every part.  The streaming submits
+ * return the envelope samples produced, which every part must agree on (ACB_ERR_CUDA otherwise).
+ * Stream / channel indices in the API and in the messages are global; messages are merged into the emission order one
+ * context gives: u8 IQ (block, stream, channel, time; rtl.c:357-360), the streaming kinds (emission group, stream,
+ * channel, time) with the groups of acb_multi_set_emission_groups (acb_set_emission_groups's units and rule), which the
+ * multi-context tracks itself; acb_multi_reset restarts them with the parts.  cfg->device is ignored, `devices` names the
  * CUDA ordinals (repeats allowed: two contexts on one GPU).  ACB_MAXSTREAMS applies to each part: a stream split
  * accepts up to ndev * 65535 streams (the parts differ by at most one stream), a channel split 65535; a part over the
- * limit fails acb_multi_create with ACB_ERR_ARG. */
+ * limit fails acb_multi_create with ACB_ERR_ARG.  Devices beyond the number of streams (channels) stay idle. */
 typedef struct acb_multi acb_multi_t;
 enum { ACB_MULTI_SPLIT_STREAMS = 0, ACB_MULTI_SPLIT_CHANNELS = 1 };
 int  acb_multi_create(const acb_config_t *cfg, const int *devices, int ndev, int mode, acb_multi_t **out);
@@ -422,6 +436,12 @@ int  acb_multi_set_plan(acb_multi_t *m, int stream, const unsigned *freqs_hz, in
 int  acb_multi_set_wf(acb_multi_t *m, int stream, const float *wf, int nch);
 int  acb_multi_reset(acb_multi_t *m);
 int  acb_multi_submit_host(acb_multi_t *m, const uint8_t *iq, size_t stream_stride, int nblk);
+int  acb_multi_set_plan_air(acb_multi_t *m, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out);
+int  acb_multi_set_plan_cs16(acb_multi_t *m, int stream, const unsigned *freqs_hz, int nch, int variant, unsigned fc_hz, unsigned *fc_out);
+int  acb_multi_submit_real_host(acb_multi_t *m, const float *x, size_t stream_stride_samples, size_t nsamples);
+int  acb_multi_submit_cs16_host(acb_multi_t *m, const int16_t *iq, size_t stream_stride_samples, size_t nsamples);
+int  acb_multi_submit_cs16_planar_host(acb_multi_t *m, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples, size_t nsamples);
+int  acb_multi_set_emission_groups(acb_multi_t *m, int unit, uint64_t period);
 int  acb_multi_collect(acb_multi_t *m);
 int  acb_multi_sync(acb_multi_t *m);
 int  acb_multi_drain(acb_multi_t *m, acb_msg_t *out, int max);
