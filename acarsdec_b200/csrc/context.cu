@@ -319,12 +319,21 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	memset(&c->stats, 0, sizeof(c->stats));
 	*out = c;
 
-	CU(cudaStreamCreateWithFlags(&c->s_copy, cudaStreamNonBlocking));
-	CU(cudaStreamCreateWithFlags(&c->s_comp, cudaStreamNonBlocking));
-	CU(cudaStreamCreateWithFlags(&c->s_dem, cudaStreamNonBlocking));
-	CU(cudaStreamCreateWithFlags(&c->s_fec, cudaStreamNonBlocking));
+	{
+		/* K2 and K3 are small, latency bound and on the serial chain of the pipeline (K2(i+1) waits for K2(i), K1(i+NPIPE)
+		 * for K2(i)'s envelope buffer); K1 is the throughput kernel that fills whatever is left.  So the demod, FEC and
+		 * read-back streams get the greatest priority and the channelizer and input-copy streams the least: when an SM
+		 * has room, a waiting K2 CTA is dispatched before the next K1 CTA.  Priority only orders the dispatch of CTAs;
+		 * it pre-empts nothing. */
+		int least = 0, greatest = 0;
+		CU(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+		CU(cudaStreamCreateWithPriority(&c->s_copy, cudaStreamNonBlocking, least));
+		CU(cudaStreamCreateWithPriority(&c->s_comp, cudaStreamNonBlocking, least));
+		CU(cudaStreamCreateWithPriority(&c->s_dem, cudaStreamNonBlocking, greatest));
+		CU(cudaStreamCreateWithPriority(&c->s_fec, cudaStreamNonBlocking, greatest));
+		CU(cudaStreamCreateWithPriority(&c->s_d2h, cudaStreamNonBlocking, greatest));
+	}
 	CU(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
-	CU(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
 	CU(cudaEventCreate(&c->mark[0]));
 	CU(cudaEventCreate(&c->mark[1]));
 	const size_t in_bytes = (size_t)cfg->nstreams * cfg->max_blocks * c->blk_bytes;

@@ -517,9 +517,9 @@ static int launch_channelize_real2(const void *in, size_t stream_stride, const v
 	const size_t smem = (size_t)C2::STAGES * C2::STAGE_BYTES;
 	cudaError_t e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) return (int)e;
-	/* both kernels ask for the largest shared-memory carve-out: an SM's L1/shared split only
-	 * changes when the SM is idle, so kernels that prefer different splits cannot be co-resident
-	 * — and the demod of submit i is meant to run underneath the channelizer of submit i+1 */
+	/* the largest shared-memory carve-out: the staging ring is this kernel's working set.  (Kernels that prefer
+	 * different splits do share an SM — the demod of submit i runs underneath the channelizer of submit i+1 whatever
+	 * the two ask for, see launch_channelize_iq4.) */
 	e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 	if (e != cudaSuccess) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
@@ -536,8 +536,11 @@ static int launch_channelize_iq4(const void *in, size_t stream_stride, const flo
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	/* a quarter of the shared-memory maximum, the rest L1: every lane of a row load touches its own 128-byte line, and
-	 * with the 28 KB of L1 the largest carve-out leaves, the kernel ran 1.2x slower (DESIGN.md §4).  The demodulator's
-	 * CTAs still fit beside it (5 KB per K1 CTA). */
+	 * with the 28 KB of L1 the largest carve-out leaves, the kernel ran 1.2x slower (DESIGN.md §4).  The demodulator runs
+	 * underneath this kernel and asks for a larger configuration, sized for its own CTAs plus three of these (4 KB + 1 KB
+	 * reserved each; the whole budget, registers included, is at launch_demod_t).  Kernels of different preferences do
+	 * share an SM: with 100 KB asked for here instead, neither this kernel alone nor the pipelined step moved (13.59
+	 * against 13.54 ms, 15.35 against 15.31 ms; H100 SXM 700 W, 4224 streams x 8 blocks). */
 	cudaError_t e = cudaFuncSetAttribute(k_channelize_iq4<MODE, OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, 25);
 	if (e != cudaSuccess) return (int)e;
 	dim3 grid(nblk * (OUTBLK / IQ4_ROWS), nstreams, ngrp);
@@ -2982,6 +2985,40 @@ k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsam
 	for (int k = 0; k < FLEN; k++) { st->inb_re[k] = sm.ring[k][grp].x; st->inb_im[k] = sm.ring[k][grp].y; }
 }
 
+/* SM count and shared memory per SM of the current device, asked per launch: contexts of one process may sit on
+ * different devices */
+static void demod_sm_limits(int &sm_count, int &smem_per_sm)
+{
+	int dev = 0;
+	sm_count = smem_per_sm = 0;
+	if (cudaGetDevice(&dev) == cudaSuccess) {
+		cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
+		cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+	}
+	if (sm_count <= 0) sm_count = 132;
+	if (smem_per_sm <= 0) smem_per_sm = 228 * 1024;
+}
+
+/* Residency budget of K2 beside the exact IQ channelizer (tools/residency_budget.py prints it from the built library,
+ * tests/test_residency_budget.py holds it).  The demod of submit i runs underneath the channelizer of submit i+1, on a
+ * stream of greater priority (context.cu): a K2 CTA that fits is dispatched before the next K1 CTA.
+ *   registers: k_channelize_iq4 allocates 160 x 128 = 20 480 per CTA, three CTAs leave 4 096 of the SM's 65 536.  One
+ *              retired K1 CTA plus that spare is 24 576: six one-warp K2 CTAs at 128 registers per thread, eight (the
+ *              share of an SM at 4224 streams x 8 channels) at 96 — hence launch_demod_one_lane's capped form.
+ *   shared:    K2 8 304 B (one lane per chain) + 1 KB reserved per CTA; K1 4 KB + 1 KB.
+ * K2 asks for the smallest shared-memory configuration that holds its CTAs of one SM (at most 16: the registers allow
+ * no more) beside three K1 CTAs — 100 KB for eight — and leaves the rest to L1, as K1 does (launch_channelize_iq4).  The
+ * envelope K2 reads comes through L1: asking for the largest carve-out (28 KB of L1) made it 1.1x slower alone (2.58
+ * against 2.33 ms, H100 SXM 700 W, 4224 streams x 8 blocks) and the pipelined step 3 % slower (15.9 against 15.5 ms); a
+ * configuration too small for its CTAs (64 KB: six fit) made it 1.6x slower alone.
+ * Launches of fewer than four warps per SM (not one per scheduler) keep the largest carve-out: there K2's serial chain is
+ * the whole step and K1 is small, and a K1 that runs faster beside it only takes issue slots from it (one stream of 256
+ * channels, K = 1600, 513 taps: K1 0.21 instead of 0.28 ms, K2 0.67 instead of 0.58 ms, the step 15 % slower). */
+constexpr int DEMOD_SMEM_RESERVED = 1024;                       /* per CTA, the system's */
+constexpr int DEMOD_SMEM_BESIDE = 3 * (4096 + DEMOD_SMEM_RESERVED);   /* three k_channelize_iq4<u8> CTAs */
+constexpr int DEMOD_MAX_WARPS_PER_SM = 16;
+constexpr int DEMOD_MIN_WARPS_SHARING = 4;                      /* per SM: below, K2 is the step and keeps the largest carve-out */
+
 template <int LANES, bool F2F, bool PIN, int MINB = 1>
 static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
                           RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
@@ -2990,7 +3027,13 @@ static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, i
 	const int wps = (nch + CPW - 1) / CPW;
 	const long long nchain = (long long)nstreams * nch;
 	const int grid = (int)((nchain + CPW - 1) / CPW);    /* one warp per CTA so that chains spread over all SMs */
-	cudaError_t e = cudaFuncSetAttribute(k_demod2<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+	int sm_count, smem_per_sm;
+	demod_sm_limits(sm_count, smem_per_sm);
+	const long long per_sm = std::min<long long>((grid + sm_count - 1) / sm_count, DEMOD_MAX_WARPS_PER_SM);
+	const long long need = per_sm * ((long long)sizeof(DemodShared<CPW>) + DEMOD_SMEM_RESERVED) + DEMOD_SMEM_BESIDE;
+	const int carve = per_sm < DEMOD_MIN_WARPS_SHARING ? (int)cudaSharedmemCarveoutMaxShared
+	                                                   : (int)std::min<long long>(100, (need * 100 + smem_per_sm - 1) / smem_per_sm);
+	cudaError_t e = cudaFuncSetAttribute(k_demod2<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
 	if (e != cudaSuccess) return (int)e;
 	k_demod2<LANES, F2F, PIN, MINB><<<grid, 32, 0, stream>>>(st, dm, nsamp, nch, nstreams, wps, ring, ctl, cap);
 	return (int)cudaGetLastError();
@@ -3004,12 +3047,30 @@ template <int LANES, bool F2F>
 static int launch_demod_pinned(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
                                RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
 {
-	int dev = 0, sm_count = 0;               /* asked per launch: contexts of one process may sit on different devices */
-	if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0)
-		sm_count = 132;
+	int sm_count, smem_per_sm;
+	demod_sm_limits(sm_count, smem_per_sm);
 	const long long warps = ((long long)nstreams * nch * LANES + 31) / 32;
 	return warps <= 8LL * sm_count ? launch_demod_t<LANES, F2F, true, 1>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream)
 	                               : launch_demod_t<LANES, F2F, true, 0>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream);
+}
+
+/* The one-lane form in two register budgets.  Left alone ptxas takes 128 registers per thread; of those CTAs six fit
+ * into the registers one retired K1 CTA frees (launch_demod_t), so with more than six warps per SM the rest wait for a
+ * second K1 CTA to retire and K1 is left with one CTA of its three on that SM meanwhile.  __launch_bounds__(32, 20)
+ * caps the kernel at 96 registers (no spills): eight fit.  Alone it is 4 % slower (2.43 against 2.33 ms), under K1 the
+ * step is 1 % faster (15.31 against 15.48-15.60 ms, three alternated runs each, same card and shape as above). */
+constexpr int DEMOD_MINB_96REG = 20;
+constexpr int DEMOD_WARPS_PER_K1_CTA = 6;
+
+static int launch_demod_one_lane(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
+                                 RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
+{
+	int sm_count, smem_per_sm;
+	demod_sm_limits(sm_count, smem_per_sm);
+	const long long warps = ((long long)nstreams * nch + 31) / 32;
+	return warps <= (long long)DEMOD_WARPS_PER_K1_CTA * sm_count
+	           ? launch_demod_t<1, false, false, 1>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream)
+	           : launch_demod_t<1, false, false, DEMOD_MINB_96REG>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream);
 }
 
 template <int LANES>
@@ -3051,7 +3112,7 @@ int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstrea
 	case -4: return launch_demod_v1<4>(ACB_DEMOD_ARGS);
 	case 8: return launch_demod_pinned<8, false>(ACB_DEMOD_ARGS);
 	case 2: return launch_demod_pinned<2, false>(ACB_DEMOD_ARGS);
-	case 1: return launch_demod_t<1, false, false>(ACB_DEMOD_ARGS);
+	case 1: return launch_demod_one_lane(ACB_DEMOD_ARGS);
 	case 17: return launch_demod_t<1, true, false>(ACB_DEMOD_ARGS);          /* F2F bit clock at one lane */
 	case 24: return launch_demod_pinned<8, true>(ACB_DEMOD_ARGS);
 	case 20: return launch_demod_pinned<4, true>(ACB_DEMOD_ARGS);
