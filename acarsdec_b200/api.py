@@ -121,6 +121,9 @@ ABI = [
     ("acb_submit_real_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     ("acb_submit_cs16_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     ("acb_submit_cs16_planar_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_submit_real_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_submit_cs16_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
+    ("acb_submit_cs16_planar_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     ("acb_set_emission_groups", C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
     ("acb_submit_dm_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     ("acb_sync", C.c_int, [C.c_void_p]),
@@ -399,6 +402,7 @@ class Context:
     def __init__(self, K: int, nstreams: int, nch: int, max_blocks: int, device: int = 0, flags: int = 0, taps: int = 0):
         self.lib = load()
         self.K, self.nstreams, self.nch, self.max_blocks = K, nstreams, nch, max_blocks
+        self.device = device
         self.block_bytes = OUTBLK * K * 2
         cfg = Config(device, K, nstreams, nch, max_blocks, flags, taps)
         h = C.c_void_p()
@@ -503,6 +507,45 @@ class Context:
         assert self._stream_stride(xq, 2, stream_stride) == stride
         return _check(self.lib, self.lib.acb_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, stride, xi.shape[1]))
 
+    # the streaming submits with the input in device memory: pointers, `nsamples` and the stream stride in samples, as the
+    # C calls take them; each returns the envelope samples produced per channel
+    def submit_real_device(self, x_dev: int, nsamples: int, stream_stride: int) -> int:
+        return _check(self.lib, self.lib.acb_submit_real_device(self.h, x_dev, stream_stride, nsamples))
+
+    def submit_cs16_device(self, iq_dev: int, nsamples: int, stream_stride: int) -> int:
+        return _check(self.lib, self.lib.acb_submit_cs16_device(self.h, iq_dev, stream_stride, nsamples))
+
+    def submit_cs16_planar_device(self, xi_dev: int, xq_dev: int, nsamples: int, stream_stride: int) -> int:
+        return _check(self.lib, self.lib.acb_submit_cs16_planar_device(self.h, xi_dev, xq_dev, stream_stride, nsamples))
+
+    def submit_tensor(self, x, xq=None) -> int:
+        """The device submits from torch CUDA tensors: float32 (nstreams, n) for a real-input context, int16
+        (nstreams, n, 2) interleaved or two int16 (nstreams, n) planes (x = I, xq = Q) for a CS16 context.  Rows may be
+        views into wider rows (their pitch is the stream stride); samples within a row are contiguous."""
+        import torch
+        for t in (x,) if xq is None else (x, xq):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device.index == self.device):
+                raise TypeError(f"torch tensors on cuda:{self.device} expected; host arrays go to submit_real / submit_cs16")
+        if xq is not None:
+            ok = x.dtype == xq.dtype == torch.int16 and x.dim() == 2 and x.shape == xq.shape and x.stride() == xq.stride()
+            layout = "two int16 (nstreams, n) planes of one shape and stride"
+        elif x.dtype == torch.float32:
+            ok, layout = x.dim() == 2, "float32 (nstreams, n)"
+        else:
+            ok = x.dtype == torch.int16 and x.dim() == 3 and x.shape[2] == 2 and x.stride(2) == 1
+            layout = "float32 (nstreams, n) or int16 (nstreams, n, 2)"
+        per = 2 if x.dim() == 3 else 1                       # tensor elements per sample: CS16 interleaved carries I and Q
+        n = x.shape[1]
+        ok = ok and x.shape[0] == self.nstreams and (n <= 1 or x.stride(1) == per) and x.stride(0) % per == 0
+        if not ok:
+            raise ValueError(f"expected {layout}, {self.nstreams} streams, samples contiguous within a row")
+        stride = x.stride(0) // per if x.shape[0] > 1 else n
+        if xq is not None:
+            return self.submit_cs16_planar_device(x.data_ptr(), xq.data_ptr(), n, stride)
+        if x.dtype == torch.float32:
+            return self.submit_real_device(x.data_ptr(), n, stride)
+        return self.submit_cs16_device(x.data_ptr(), n, stride)
+
     def set_emission_groups(self, unit: int, period: int = 0) -> None:
         """unit: 0 per submit, 1 every `period` envelope samples, 2 per transfer of `period` input samples."""
         _check(self.lib, self.lib.acb_set_emission_groups(self.h, unit, period))
@@ -605,7 +648,8 @@ class Context:
         _check(self.lib, self.lib.acb_set_plan_at(self.h, stream, f.ctypes.data, len(f), int(fc_hz)))
 
     def wait_event(self, cuda_event: int) -> None:
-        """Order the next submit_device behind a cudaEvent_t of another stream (torch.cuda.Event.cuda_event)."""
+        """Order the next submit_device (and the next streaming device submit's read of its input) behind a cudaEvent_t of
+        another stream (torch.cuda.Event.cuda_event)."""
         _check(self.lib, self.lib.acb_wait_event(self.h, cuda_event))
 
 

@@ -116,6 +116,10 @@ int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, co
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
 int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_stride, uint32_t *out, size_t out_stride,
                            size_t nsamples, int nstreams, CUstream_st *stream);
+/* device submits of the streaming kinds: `nsamples` 4-byte samples per stream from a (b = NULL) or from the int16 planes a, b
+ * (interleaved on the way), source rows `src_stride` samples apart, to out + s*out_stride (any 4-byte alignment) */
+int launch_append4(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, size_t nsamples, int nstreams,
+                   CUstream_st *stream);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
 

@@ -157,6 +157,9 @@ struct acb_ctx {
 	bool real_used[2];
 	int16_t *d_planar;           /* CS16 planar input: both planes of one submit, interleaved on the device */
 	size_t planar_cap;           /* int16 elements per plane and stream */
+	cudaStream_t s_order;        /* streaming kinds: collects the acb_wait_event waits for the next device submit's append */
+	cudaEvent_t ev_order;        /* recorded on s_order behind the last of those waits */
+	bool order_pending;          /* ev_order has a wait the copy stream has not yet been ordered behind */
 	int group_unit;              /* ACB_GROUP_*: how the streaming front-ends' frames are grouped for emission */
 	unsigned long long group_period;
 };
@@ -302,6 +305,9 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->planar_cap = 0;
 	c->ev_real_copied = nullptr;
 	c->ev_real_free[0] = c->ev_real_free[1] = nullptr;
+	c->s_order = nullptr;
+	c->ev_order = nullptr;
+	c->order_pending = false;
 	c->carry = 0;
 	c->real_buf = 0;
 	c->group_unit = ACB_GROUP_SUBMIT;
@@ -353,7 +359,11 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming));
 		CU(cudaEventCreateWithFlags(&c->ev_consumed[i], cudaEventDisableTiming));
 	}
-	if (c->real_input) CU(cudaEventCreateWithFlags(&c->ev_real_copied, cudaEventDisableTiming));
+	if (c->real_input) {
+		CU(cudaEventCreateWithFlags(&c->ev_real_copied, cudaEventDisableTiming));
+		CU(cudaStreamCreateWithFlags(&c->s_order, cudaStreamNonBlocking));
+		CU(cudaEventCreateWithFlags(&c->ev_order, cudaEventDisableTiming));
+	}
 	/* u8 IQ history: its own buffer (acb_submit_device copies no input).  The streaming kinds keep theirs in front of
 	 * the carried remainder in d_real. */
 	if (c->hpad && !c->real_input) CU(cudaMalloc(&c->d_hist, (size_t)cfg->nstreams * c->hpad * 2));
@@ -474,6 +484,8 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 		for (auto &t : c->inflight) { cudaEventDestroy(t.ev.a); cudaEventDestroy(t.ev.b); cudaEventDestroy(t.ev.b2); cudaEventDestroy(t.ev.c); }
 		for (auto &e : c->ev_free) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); cudaEventDestroy(e.b2); cudaEventDestroy(e.c); }
 		if (c->ev_real_copied) cudaEventDestroy(c->ev_real_copied);
+		if (c->ev_order) cudaEventDestroy(c->ev_order);
+		if (c->s_order) cudaStreamDestroy(c->s_order);
 		cudaFree(c->d_planar);
 		cudaFree(c->d_hist);
 		cudaFree(c->d_wf); cudaFree(c->d_state);
@@ -1065,8 +1077,9 @@ std::vector<unsigned long long> acb::stream_groups(int unit, unsigned long long 
 
 /* 4-byte samples (float32 real or int16 I,Q) of arbitrary count: appended behind the carried
  * remainder in d_real[b]; `x2` != NULL means planar int16 input (x = I plane, x2 = Q plane), which
- * two strided copies interleave on the way to the device */
-static int submit4(acb_ctx *c, const void *x, const void *x2, size_t stride_samples, size_t nsamples)
+ * is interleaved on the way.  `dev`: the input is in device memory (the device calls) and one append
+ * kernel moves it; otherwise strided host copies bring it over.  Everything else is the same for both. */
+static int submit4(acb_ctx *c, const void *x, const void *x2, bool dev, size_t stride_samples, size_t nsamples)
 {
 	if (int r = ctx_use(c)) return r;
 	const size_t K = (size_t)c->cfg.K, total = c->carry + nsamples, hp = (size_t)c->hpad;
@@ -1080,7 +1093,17 @@ static int submit4(acb_ctx *c, const void *x, const void *x2, size_t stride_samp
 	 * taps > K: the first hp samples of each stream are its history, rows start behind them. */
 	float *const buf0 = c->d_real[b], *const buf = buf0 + hp;
 	if (c->real_used[b]) CU(cudaStreamWaitEvent(c->s_copy, c->ev_real_free[b], 0));
-	if (!x2) {
+	if (dev) {
+		/* acb_wait_event: the caller's producer must be done before the append reads the input */
+		if (c->order_pending) {
+			CU(cudaStreamWaitEvent(c->s_copy, c->ev_order, 0));
+			c->order_pending = false;
+		}
+		int r = launch_append4(x, x2, stride_samples, reinterpret_cast<uint32_t *>(buf + c->carry), c->real_cap, nsamples,
+		                       c->cfg.nstreams, c->s_copy);
+		if (r) return fail(ACB_ERR_CUDA, "append launch: %s", cudaGetErrorString((cudaError_t)r));
+		c->stats.kernel_launches++;
+	} else if (!x2) {
 		CU(cudaMemcpy2DAsync(buf + c->carry, c->real_cap * sizeof(float), x, stride_samples * sizeof(float),
 		                     nsamples * sizeof(float), c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
 	} else {
@@ -1128,21 +1151,63 @@ extern "C" int acb_submit_real_host(acb_ctx_t *c, const float *x, size_t stride_
 {
 	if (!c || !x) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_F32REAL) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_REAL_INPUT");
-	return submit4(c, x, nullptr, stride_samples, nsamples);
+	return submit4(c, x, nullptr, false, stride_samples, nsamples);
 }
 
 extern "C" int acb_submit_cs16_host(acb_ctx_t *c, const int16_t *iq, size_t stride_samples, size_t nsamples)
 {
 	if (!c || !iq) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
-	return submit4(c, iq, nullptr, stride_samples, nsamples);
+	return submit4(c, iq, nullptr, false, stride_samples, nsamples);
 }
 
 extern "C" int acb_submit_cs16_planar_host(acb_ctx_t *c, const int16_t *xi, const int16_t *xq, size_t stride_samples, size_t nsamples)
 {
 	if (!c || !xi || !xq) return fail(ACB_ERR_ARG, "null argument");
 	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
-	return submit4(c, xi, xq, stride_samples, nsamples);
+	return submit4(c, xi, xq, false, stride_samples, nsamples);
+}
+
+/* The device calls take device memory of the context's device, or managed memory, only: host memory (pinned or
+ * pageable) has the host calls, and another device's memory would be read over the peer link if at all. */
+static int check_device_input(acb_ctx *c, const void *p, size_t align)
+{
+	if ((uintptr_t)p % align) return fail(ACB_ERR_ARG, "device input must be %zu-byte aligned", align);
+	cudaPointerAttributes a;
+	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+		cudaGetLastError();                         /* not sticky: clear it so the next call does not report it */
+		return fail(ACB_ERR_ARG, "input is not memory CUDA knows");
+	}
+	if (a.type == cudaMemoryTypeManaged || (a.type == cudaMemoryTypeDevice && a.device == c->cfg.device)) return ACB_OK;
+	if (a.type == cudaMemoryTypeDevice)
+		return fail(ACB_ERR_ARG, "input is on device %d, the context on device %d", a.device, c->cfg.device);
+	return fail(ACB_ERR_ARG, "input is host memory: use the host call");
+}
+
+extern "C" int acb_submit_real_device(acb_ctx_t *c, const float *x_dev, size_t stride_samples, size_t nsamples)
+{
+	if (!c || !x_dev) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_F32REAL) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_REAL_INPUT");
+	if (int r = check_device_input(c, x_dev, 4)) return r;
+	return submit4(c, x_dev, nullptr, true, stride_samples, nsamples);
+}
+
+extern "C" int acb_submit_cs16_device(acb_ctx_t *c, const int16_t *iq_dev, size_t stride_samples, size_t nsamples)
+{
+	if (!c || !iq_dev) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	if (int r = check_device_input(c, iq_dev, 4)) return r;
+	return submit4(c, iq_dev, nullptr, true, stride_samples, nsamples);
+}
+
+extern "C" int acb_submit_cs16_planar_device(acb_ctx_t *c, const int16_t *xi_dev, const int16_t *xq_dev, size_t stride_samples,
+                                             size_t nsamples)
+{
+	if (!c || !xi_dev || !xq_dev) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	if (int r = check_device_input(c, xi_dev, 2)) return r;
+	if (int r = check_device_input(c, xq_dev, 2)) return r;
+	return submit4(c, xi_dev, xq_dev, true, stride_samples, nsamples);
 }
 
 extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, int variant, unsigned fc_hz, unsigned *fc_out)
@@ -1232,6 +1297,14 @@ extern "C" int acb_wait_event(acb_ctx_t *c, void *cuda_event)
 	if (!c || !cuda_event) return fail(ACB_ERR_ARG, "null argument");
 	if (int r = ctx_use(c)) return r;
 	CU(cudaStreamWaitEvent(c->s_comp, (cudaEvent_t)cuda_event, 0));
+	if (c->real_input) {
+		/* The streaming device submits read their input on the copy stream.  The wait is taken now, on a stream of its
+		 * own, so that it is the event as recorded at this call that counts, and the host submits' copies on the copy
+		 * stream are not held up by it; the next device submit orders its append behind ev_order. */
+		CU(cudaStreamWaitEvent(c->s_order, (cudaEvent_t)cuda_event, 0));
+		CU(cudaEventRecord(c->ev_order, c->s_order));
+		c->order_pending = true;
+	}
 	return ACB_OK;
 }
 

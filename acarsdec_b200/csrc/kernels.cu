@@ -2450,6 +2450,47 @@ int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_st
 	return (int)cudaGetLastError();
 }
 
+/* The device submits of the streaming kinds: stream s's `nsamples` new 4-byte samples land behind its history and carried
+ * remainder, out[s][i] = a[s][i] (float32 real or interleaved CS16), or out[s][i] = (a[s][i], b[s][i]) from the caller's
+ * separate I and Q planes (PLANAR).  The source has any 4-byte (planes: 2-byte) alignment and stride; the destination
+ * row starts at hpad + carry samples, generally not on 16 bytes, so a head of up to 3 samples and a tail of up to 3 go
+ * singly and every whole 16-byte unit between them is one vector store.  Pure data movement, read once, written once. */
+template <bool PLANAR>
+__global__ void __launch_bounds__(256)
+k_append4(const void *__restrict__ a, const void *__restrict__ b, size_t src_stride, uint32_t *__restrict__ out,
+          size_t out_stride, size_t nsamples)
+{
+	const int s = blockIdx.y;
+	const uint32_t *x = reinterpret_cast<const uint32_t *>(a) + (size_t)s * src_stride;
+	const uint16_t *pi = reinterpret_cast<const uint16_t *>(a) + (size_t)s * src_stride;
+	const uint16_t *pq = reinterpret_cast<const uint16_t *>(b) + (size_t)s * src_stride;
+	uint32_t *o = out + (size_t)s * out_stride;
+	auto at = [&](size_t i) -> uint32_t {
+		if constexpr (PLANAR) return (uint32_t)pi[i] | ((uint32_t)pq[i] << 16);
+		else return x[i];
+	};
+	const size_t head = min(nsamples, (size_t)(((16 - ((uintptr_t)o & 15)) & 15) / 4));
+	const size_t nvec = (nsamples - head) / 4, tail0 = head + 4 * nvec;
+	const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (size_t)gridDim.x * blockDim.x;
+	uint4 *ov = reinterpret_cast<uint4 *>(o + head);
+	for (size_t v = tid; v < nvec; v += nth) {
+		const size_t i = head + 4 * v;
+		ov[v] = make_uint4(at(i), at(i + 1), at(i + 2), at(i + 3));
+	}
+	if (tid < head) o[tid] = at(tid);
+	if (tid < nsamples - tail0) o[tail0 + tid] = at(tail0 + tid);
+}
+
+int launch_append4(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, size_t nsamples, int nstreams,
+                   cudaStream_t stream)
+{
+	if (nsamples == 0) return 0;
+	const unsigned gx = (unsigned)std::min<size_t>((nsamples / 4 + 255) / 256 + 1, 1184);
+	if (b) k_append4<true><<<dim3(gx, nstreams), 256, 0, stream>>>(a, b, src_stride, out, out_stride, nsamples);
+	else k_append4<false><<<dim3(gx, nstreams), 256, 0, stream>>>(a, nullptr, src_stride, out, out_stride, nsamples);
+	return (int)cudaGetLastError();
+}
+
 /* Rows the pipeline kernel does not take (K that breaks 16-byte row alignment; the < 1024 rows
  * left over by a real-input submit of arbitrary length): one thread per (output, channel),
  * straight from global memory, same arithmetic.  Correctness path, not tuned. */

@@ -9,10 +9,12 @@ read-only matched filter, streams share nothing at all.
     gloo in the CPU tests) — each rank then channelizes/demodulates only its own channels.
 
 Decoded messages come back per rank and are merged in the reference's emission order
-(block-major, then stream, then channel, then time; rtl.c:357-360).
+(block-major, then stream, then channel, then time; rtl.c:357-360); for the streaming front-ends (real input,
+CS16) the emission group of acb_set_emission_groups takes the block's place.
 """
 from __future__ import annotations
 
+import bisect
 import os
 from typing import Iterable, Sequence
 
@@ -78,6 +80,39 @@ def whole_job_throughput(dist, samples_local: float, seconds_local: float, devic
     total = reduce_scalar(dist, samples_local, "sum", device)
     slowest = reduce_scalar(dist, seconds_local, "max", device)
     return total / slowest
+
+
+GROUP_SUBMIT, GROUP_OUTPUTS, GROUP_INPUT = 0, 1, 2      # acb_set_emission_groups's units
+
+
+def stream_groups(unit: int, period: int, K: int, pos: int, nout: int) -> list:
+    """Emission-group starts of a streaming submit that produced envelope samples [pos, pos + nout), as a context cuts
+    them (acb_set_emission_groups): the first is pos, then one every `period` outputs counted from the stream start
+    (GROUP_OUTPUTS), or one per transfer of `period` input samples (GROUP_INPUT: output m completes with input sample
+    (m+1)K - 1, so transfer t starts a group at output t*period // K).  A submit that produced no row has no group."""
+    if nout <= 0:
+        return []
+    g, hi = [pos], pos + nout
+    if unit == GROUP_OUTPUTS:
+        b = (pos // period + 1) * period
+        while b < hi:
+            g.append(b)
+            b += period
+    elif unit == GROUP_INPUT:
+        t = pos * K // period + 1                          # transfers that start after output `pos` began
+        while True:
+            b = t * period // K                            # first output completed inside transfer t
+            if b >= hi:
+                break
+            if b > g[-1]:
+                g.append(b)
+            t += 1
+    return g
+
+
+def group_of(starts: Sequence[int], pos: int) -> int:
+    """Index of a message's emission group: the last start at or before its pos (`starts` ascending)."""
+    return bisect.bisect_right(starts, pos)
 
 
 def merge_messages(per_rank: Sequence[Iterable], key=lambda m: (m.block, m.stream, m.chn, m.pos)):

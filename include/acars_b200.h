@@ -329,6 +329,23 @@ int acb_submit_cs16_planar_host(acb_ctx_t *ctx, const int16_t *xi, const int16_t
  *     covered the submit.  Submits that produced rows are covered in call order, one per acb_collect (the oldest first),
  *     and all of them by acb_sync.  A submit that produced no row (returned 0) is covered only by the next acb_sync.
  * A refused call (negative return) has read nothing, and the carried remainder is unchanged. */
+/* The same three with the input already in device memory (a GPU-native source, or the broadcast buffer of a wide stream
+ * served by several GPUs): arguments, return value, carried remainder, taps > K history, emission groups and every
+ * channelizer form are the host calls', and a context may mix host and device submits of its kind freely — the result is
+ * the one all-host submits give.  A small kernel appends each stream's samples behind its carried remainder on the
+ * device: no host round trip, no synchronisation, no allocation.
+ *   - Where the input may live: device memory of the context's device, or managed memory (cudaPointerGetAttributes
+ *     decides).  Host memory, pinned or pageable, and another device's memory are refused with ACB_ERR_ARG.  The
+ *     interleaved forms need 4-byte aligned input, the planar planes 2-byte aligned ones.
+ *   - The host calls' refusals hold unchanged (wrong context kind, nsamples 0 or beyond max_blocks*1024*K, a stride
+ *     smaller than nsamples with several streams); a refused call reads nothing and leaves the carry unchanged.
+ *   - Input lifetime: that of pinned host memory above.  The input may be overwritten once an acb_collect or acb_sync
+ *     has covered the submit; a submit that returned 0 is covered only by the next acb_sync.
+ *   - Ordering: acb_wait_event orders the next device submit's read of its input behind the event (see there). */
+int acb_submit_real_device(acb_ctx_t *ctx, const float *x_dev, size_t stream_stride_samples, size_t nsamples);
+int acb_submit_cs16_device(acb_ctx_t *ctx, const int16_t *iq_dev, size_t stream_stride_samples, size_t nsamples);
+int acb_submit_cs16_planar_device(acb_ctx_t *ctx, const int16_t *xi_dev, const int16_t *xq_dev,
+                                  size_t stream_stride_samples, size_t nsamples);
 /* Emission order of the streaming front-ends (SURVEY H5).  The reference runs demodMSK channel by channel on
  * whatever a transfer (air.c:336) or a full dm_buffer (soapy.c:247: 1024 outputs; sdrplay.c:229: 512) delivered, so
  * its messages leave in (group, channel, time) order.  A submit may carry many such groups; tell the context how
@@ -343,7 +360,11 @@ int acb_set_emission_groups(acb_ctx_t *ctx, int unit, uint64_t period);
  * dm[(s*nsamp + n)*nch + c], fed straight to the demodulator (no channelizer). */
 int acb_submit_dm_host(acb_ctx_t *ctx, const float *dm, int nsamp);
 /* Order the next acb_submit_device behind work of ANOTHER CUDA stream: `cuda_event` is a cudaEvent_t recorded there
- * (e.g. behind the NCCL broadcast that fills the input buffer; torch.cuda.Event.cuda_event).  No host sync. */
+ * (e.g. behind the NCCL broadcast that fills the input buffer; torch.cuda.Event.cuda_event).  No host sync.
+ * On real-input and CS16 contexts it also orders the next acb_submit_real_device / acb_submit_cs16_device /
+ * acb_submit_cs16_planar_device's read of its input behind the event as recorded at this call (the host submits'
+ * copies are not held up by it).  Every later submit is ordered behind that one, so one wait covers a device buffer
+ * for as long as it is not refilled. */
 int acb_wait_event(acb_ctx_t *ctx, void *cuda_event);
 /* Wait for the OLDEST submit still in flight only (at most three are), run the block FEC on its
  * frames and queue the survivors; later submits keep running.  This is what lets the H2D copy
@@ -425,7 +446,10 @@ int acb_get_stats(acb_ctx_t *ctx, acb_stats_t *out, int reset);
  * multi-context tracks itself; acb_multi_reset restarts them with the parts.  cfg->device is ignored, `devices` names the
  * CUDA ordinals (repeats allowed: two contexts on one GPU).  ACB_MAXSTREAMS applies to each part: a stream split
  * accepts up to ndev * 65535 streams (the parts differ by at most one stream), a channel split 65535; a part over the
- * limit fails acb_multi_create with ACB_ERR_ARG.  Devices beyond the number of streams (channels) stay idle. */
+ * limit fails acb_multi_create with ACB_ERR_ARG.  Devices beyond the number of streams (channels) stay idle.
+ * Input comes from the host only: a device pointer belongs to one GPU.  Several GPUs reading one wide stream from
+ * device memory broadcast it and give each context its copy (acb_wait_event + the device submits; Python:
+ * acarsdec_b200.wide.WideStream). */
 typedef struct acb_multi acb_multi_t;
 enum { ACB_MULTI_SPLIT_STREAMS = 0, ACB_MULTI_SPLIT_CHANNELS = 1 };
 int  acb_multi_create(const acb_config_t *cfg, const int *devices, int ndev, int mode, acb_multi_t **out);

@@ -84,4 +84,25 @@ with api.Context(Kr, 1, 13, 1, flags=2 | api.FLAG_FAST_WIDEBAND_REAL, taps=2 * K
         ctx.submit_real(part)
     ctx.sync()
     assert ctx.stats().fast_chan_launches == 2          # the 1000-sample submit completes no row
+# the streaming kinds' device submits: one of each kind behind a carry of 77 samples (a destination offset that is not on
+# 16 bytes), the source rows 5 samples wider than the input, taps > K (the history in front of the rows)
+import torch  # noqa: E402
+for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
+    with api.Context(Kd, 2, 3, 1, flags=fl, taps=2 * Kd + 3) as ctx:
+        for s in range(2):
+            ctx.set_plan_air(s, fda) if kind == "real" else ctx.set_plan_cs16(s, fd[:3], 0)
+        n = 3 * Kd + 7
+        if kind == "real":
+            dev = torch.randn((2, n + 5), device="cuda") * 100
+            assert ctx.submit_real((dev[:, :77].cpu().numpy()).copy()) == 0
+            assert ctx.submit_tensor(dev[:, :n]) == 3
+        else:
+            dev = torch.randint(-3000, 3000, (2, n + 5, 2), dtype=torch.int16, device="cuda")
+            assert ctx.submit_cs16(dev[:, :77].cpu().numpy().copy()) == 0
+            if kind == "cs16":
+                assert ctx.submit_tensor(dev[:, :n]) == 3
+            else:
+                planes = dev.permute(2, 0, 1).contiguous()
+                assert ctx.submit_tensor(planes[0, :, :n], planes[1, :, :n]) == 3
+        ctx.sync()
 print("sanitize run ok", n1, n3, n4, n5)
