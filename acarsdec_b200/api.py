@@ -19,6 +19,7 @@ OUTBLK = 1024
 TXTMAX = 250
 FLAG_FAST_WIDEBAND = 64          # ACB_FLAG_FAST_WIDEBAND: the fast forms for any K % 8 == 0 and any channel count
 FLAG_FAST_WIDEBAND_REAL = 128    # ACB_FLAG_FAST_WIDEBAND_REAL: the same for real input (air.c)
+FLAG_DECODE_STATS = 256          # ACB_FLAG_DECODE_STATS: per-chain decode statistics (Context.decode_stats)
 
 
 class Config(C.Structure):
@@ -85,6 +86,13 @@ class Stats(C.Structure):
                 ("raw_frames", C.c_uint64), ("fec_dropped", C.c_uint64), ("chan_ms", C.c_double),
                 ("demod_ms", C.c_double), ("chan_launches", C.c_uint64), ("demod_launches", C.c_uint64),
                 ("fast_chan_launches", C.c_uint64), ("frames_lost", C.c_uint64), ("host_ms", C.c_double)]
+
+
+# acb_decode_stats_t, field for field (include/acars_b200.h names the reference event each one counts)
+DECODE_STATS_FIELDS = ("preamble", "started", "txt_parity", "txt_long", "txt_missed_end", "emitted",
+                       "fec_short", "fec_parity_excess", "fec_parity", "fec_crc", "fec_fixed", "fec_unfixable",
+                       "fec_parity_problem", "delivered", "lost")
+DECODE_STATS_DTYPE = np.dtype([(f, "<u8") for f in DECODE_STATS_FIELDS])
 
 
 # every symbol include/acars_b200.h declares: (name, restype, argtypes)
@@ -167,6 +175,8 @@ ABI = [
     ("acb_get_state", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(ChanState)]),
     ("acb_set_state", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(ChanState)]),
     ("acb_get_stats", C.c_int, [C.c_void_p, C.POINTER(Stats), C.c_int]),
+    ("acb_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_multi_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_block_fec", C.c_int, [C.POINTER(Msg)]),
     ("acb_block_fec_batch", C.c_int, [C.c_void_p, C.POINTER(Msg), C.c_int, C.POINTER(C.c_int)]),
     ("acb_crc_update", C.c_uint16, [C.c_uint16, C.c_uint8]),
@@ -630,6 +640,12 @@ class Context:
         _check(self.lib, self.lib.acb_get_stats(self.h, C.byref(s), int(reset)))
         return s
 
+    def decode_stats(self, reset: bool = False) -> np.ndarray:
+        """Per-chain decode statistics (FLAG_DECODE_STATS): a DECODE_STATS_DTYPE array of shape (nstreams, nch)."""
+        out = np.zeros((self.nstreams, self.nch), dtype=DECODE_STATS_DTYPE)
+        _check(self.lib, self.lib.acb_get_decode_stats(self.h, out.ctypes.data, out.size, int(reset)))
+        return out
+
     def device_alloc(self, nbytes: int) -> int:
         p = self.lib.acb_device_alloc(self.h, nbytes)
         if not p:
@@ -743,6 +759,12 @@ class MultiContext:
         s = Stats()
         _check(self.lib, self.lib.acb_get_stats(self.lib.acb_multi_part(self.h, i), C.byref(s), int(reset)))
         return s
+
+    def decode_stats(self, reset: bool = False) -> np.ndarray:
+        """As Context.decode_stats, indexed by global stream and channel."""
+        out = np.zeros((self.nstreams, self.nch), dtype=DECODE_STATS_DTYPE)
+        _check(self.lib, self.lib.acb_multi_get_decode_stats(self.h, out.ctypes.data, out.size, int(reset)))
+        return out
 
     def sync(self) -> int:
         return _check(self.lib, self.lib.acb_multi_sync(self.h))

@@ -44,8 +44,20 @@ struct RawFrame {
 	int pad0;                         /* block-FEC status: 0 = not processed, 1 = deliver, 2 = drop */
 	unsigned long long pos, soh_pos;
 	unsigned char crc[2];
-	unsigned char pad1[6];
+	unsigned char pad1[6];            /* pad1[0]: why the block FEC ended as it did, FEC_WHY_* (k_block_fec_stats only) */
 	unsigned char txt[TXTCAP];
+};
+
+/* blk_thread's verdicts (acars.c:124-206) as k_block_fec_stats records them: a frame in the ring ends in exactly one of
+ * PARITY_EXCESS, UNFIXABLE, PARITY_PROBLEM or delivery (status 1); PARITY, CRC and FIXED are on the way there */
+enum FecWhy {
+	FEC_WHY_PARITY = 1,               /* 1..MAXPERR parity errors (acars.c:153-155) */
+	FEC_WHY_CRC = 2,                  /* CRC non-zero (acars.c:166-167) */
+	FEC_WHY_FIXED = 4,                /* "errors fixed" (acars.c:177-178, 189-190) */
+	FEC_WHY_UNFIXABLE = 8,            /* "not able to fix errors" (acars.c:172-173, 184-185) */
+	FEC_WHY_PARITY_EXCESS = 16,       /* more than MAXPERR parity errors (acars.c:145-152) */
+	FEC_WHY_PARITY_PROBLEM = 32,      /* the final parity re-check failed (acars.c:202-206) */
+	FEC_WHY_SHORT = 64                /* under 13 or over 250 bytes (acars.c:124-129; the ring holds none) */
 };
 
 struct RingCtl {
@@ -96,6 +108,11 @@ int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride
                                   const Hist &h, CUstream_st *stream);
 int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
                  RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, CUstream_st *stream);
+/* The counting form (ACB_FLAG_DECODE_STATS): the same demodulator, and chain g adds its frame synchroniser's events to
+ * counts[g * EV_COUNT + e] (frame_sm.h; the caller clears them).  Lanes 1, 2, 4 or 8 only (the default forms): anything
+ * else returns cudaErrorInvalidValue and launches nothing. */
+int launch_demod_stats(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
+                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, unsigned *counts, CUstream_st *stream);
 int demod_pick_lanes(long long nchains, int sm_count);
 bool channelize_dft_supports(int K);
 int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
@@ -114,6 +131,8 @@ int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, c
 int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
                               float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
+/* the same repair, and each frame's FEC_WHY_* in RawFrame::pad1[0] */
+int launch_block_fec_stats(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
 int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_stride, uint32_t *out, size_t out_stride,
                            size_t nsamples, int nstreams, CUstream_st *stream);
 /* device submits of the streaming kinds: `nsamples` 4-byte samples per stream from a (b = NULL) or from the int16 planes a, b

@@ -37,6 +37,7 @@
 
 #include "../../include/acars_b200.h"
 #include "acb_internal.h"
+#include "frame_sm.h"
 
 using namespace acb;
 
@@ -162,6 +163,14 @@ struct acb_ctx {
 	bool order_pending;          /* ev_order has a wait the copy stream has not yet been ordered behind */
 	int group_unit;              /* ACB_GROUP_*: how the streaming front-ends' frames are grouped for emission */
 	unsigned long long group_period;
+	/* ACB_FLAG_DECODE_STATS: per frame ring (submit in flight), the counting demod's EV_COUNT counters per chain, cleared
+	 * before its launch and read back with that submit's frames; the consumer adds them and each frame's FEC verdict to
+	 * dstats */
+	bool decode_stats;
+	std::mutex dstats_mtx;       /* guards dstats: the consumer adds to it without holding up acb_drain on mtx */
+	unsigned *d_evcnt[NPIPE];
+	unsigned *h_evcnt[NPIPE];    /* pinned */
+	std::vector<acb_decode_stats_t> dstats;      /* guarded by dstats_mtx */
 };
 
 static void consumer_main(acb_ctx *c);
@@ -250,6 +259,10 @@ static int reset_states(acb_ctx *c)
 		c->outq.clear();
 		c->outq_count = 0;
 	}
+	if (c->decode_stats) {       /* the counts go with the undrained messages: those of a reset context restart from nothing */
+		std::lock_guard<std::mutex> lk(c->dstats_mtx);
+		memset(c->dstats.data(), 0, c->dstats.size() * sizeof(acb_decode_stats_t));
+	}
 	c->overflowed = false;
 	return ACB_OK;
 }
@@ -323,6 +336,8 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->h_ring[0] = c->h_ring[1] = nullptr;
 	c->overflowed = false;
 	memset(&c->stats, 0, sizeof(c->stats));
+	c->decode_stats = (cfg->flags & ACB_FLAG_DECODE_STATS) != 0;
+	for (int i = 0; i < NPIPE; i++) c->d_evcnt[i] = nullptr, c->h_evcnt[i] = nullptr;
 	*out = c;
 
 	{
@@ -393,7 +408,10 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		 * +16 = F2F bit-clock rounding, +32 = constants not pinned, -4 / -8 = the round-1 kernel (launch_demod) */
 		if (const char *e = getenv("ACB_DEMOD_LANES")) {
 			const int v = atoi(e), l = v & 15;
-			if (v == -4 || v == -8 || (v > 0 && v < 64 && (l == 1 || l == 2 || l == 4 || l == 8))) c->demod_lanes = v;
+			/* ACB_FLAG_DECODE_STATS: the plain widths only, the forms with a counting kernel (the others keep the pick) */
+			const bool counted = v == 1 || v == 2 || v == 4 || v == 8;
+			if (c->decode_stats ? counted : (v == -4 || v == -8 || (v > 0 && v < 64 && (l == 1 || l == 2 || l == 4 || l == 8))))
+				c->demod_lanes = v;
 		}
 	}
 	if (c->fast || c->fast_ovl) {
@@ -447,6 +465,13 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaHostAlloc(&c->h_ctl[i], sizeof(RingCtl), cudaHostAllocDefault));
 	}
 	for (int i = 0; i < NPIPE; i++) CU(cudaHostAlloc(&c->h_ring[i], cap * sizeof(RawFrame), cudaHostAllocDefault));
+	if (c->decode_stats) {
+		c->dstats.assign(nchain, acb_decode_stats_t{});
+		for (int i = 0; i < NPIPE; i++) {
+			CU(cudaMalloc(&c->d_evcnt[i], nchain * EV_COUNT * sizeof(unsigned)));
+			CU(cudaHostAlloc(&c->h_evcnt[i], nchain * EV_COUNT * sizeof(unsigned), cudaHostAllocDefault));
+		}
+	}
 	c->consumer = std::thread(consumer_main, c);
 
 	float h[FLENO];
@@ -495,6 +520,7 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 			cudaFree(c->d_dm[i]); cudaEventDestroy(c->ev_k1_done[i]); cudaEventDestroy(c->ev_dm_free[i]);
 			cudaEventDestroy(c->ev_k2_done[i]); cudaEventDestroy(c->ev_ring_read[i]);
 			cudaFree(c->d_ring[i]); cudaFree(c->d_ctl[i]); cudaFreeHost(c->h_ctl[i]); cudaFreeHost(c->h_ring[i]);
+			cudaFree(c->d_evcnt[i]); cudaFreeHost(c->h_evcnt[i]);
 		}
 		cudaEventDestroy(c->mark[0]); cudaEventDestroy(c->mark[1]); cudaEventDestroy(c->ev_join);
 		cudaStreamDestroy(c->s_copy); cudaStreamDestroy(c->s_comp); cudaStreamDestroy(c->s_dem); cudaStreamDestroy(c->s_fec); cudaStreamDestroy(c->s_d2h);
@@ -647,6 +673,40 @@ static EvTriple get_events(acb_ctx *c)
  *                  if the reference served them in turn.
  * So the host-side sort/copy of submit i-1 never delays the launches of submit i+1; acb_collect / acb_sync wait for the
  * consumer to have caught up with what they collected. */
+
+/* ACB_FLAG_DECODE_STATS: a collected submit's counts into the context's table — the counting demod's per-chain
+ * events, and the verdict k_block_fec_stats gave each of its frames in the ring */
+static void add_decode_stats(acb_ctx *c, const acb_ctx::Job &job, const RawFrame *ring, const unsigned char *keep)
+{
+	std::lock_guard<std::mutex> lk(c->dstats_mtx);
+	const size_t nchain = c->dstats.size();
+	const unsigned *ev = c->h_evcnt[job.ring];
+	for (size_t g = 0; g < nchain; g++) {
+		const unsigned *e = ev + g * EV_COUNT;
+		acb_decode_stats_t &d = c->dstats[g];
+		d.preamble += e[EV_PREAMBLE];
+		d.started += e[EV_STARTED];
+		d.txt_parity += e[EV_TXT_PARITY];
+		d.txt_long += e[EV_TXT_LONG];
+		d.txt_missed_end += e[EV_TXT_MISSED_END];
+		d.emitted += e[EV_EMITTED];
+		d.fec_short += e[EV_SHORT];
+		d.lost += e[EV_LOST];
+	}
+	for (unsigned i = 0; i < job.count; i++) {
+		const RawFrame &f = ring[i];
+		const unsigned why = f.pad1[0];
+		acb_decode_stats_t &d = c->dstats[(size_t)f.stream * c->cfg.nch + f.chn];
+		d.fec_parity_excess += (why & FEC_WHY_PARITY_EXCESS) != 0;
+		d.fec_parity += (why & FEC_WHY_PARITY) != 0;
+		d.fec_crc += (why & FEC_WHY_CRC) != 0;
+		d.fec_fixed += (why & FEC_WHY_FIXED) != 0;
+		d.fec_unfixable += (why & FEC_WHY_UNFIXABLE) != 0;
+		d.fec_parity_problem += (why & FEC_WHY_PARITY_PROBLEM) != 0;
+		d.delivered += keep[i];
+	}
+}
+
 static void consume(acb_ctx *c, const acb_ctx::Job &job)
 {
 	const unsigned count = job.count;
@@ -735,6 +795,7 @@ static void consume(acb_ctx *c, const acb_ctx::Job &job)
 		fill(0, std::min(count, per));
 		for (auto &th : pool) th.join();
 	}
+	if (c->decode_stats) add_decode_stats(c, job, ring, keep.data());     /* before the job counts as done */
 	const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
 	std::lock_guard<std::mutex> lk(c->mtx);
 	c->stats.raw_frames += count;
@@ -758,7 +819,7 @@ static void consumer_main(acb_ctx *c)
 			job = std::move(c->jobs.front());
 			c->jobs.pop_front();
 		}
-		const cudaError_t e = job.count ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
+		const cudaError_t e = job.count || c->decode_stats ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
 		if (e == cudaSuccess) consume(c, job);
 		{
 			std::lock_guard<std::mutex> lk(c->mtx);
@@ -802,6 +863,9 @@ static int harvest_begin(acb_ctx *c)
 	}
 	if (count)
 		CU(cudaMemcpyAsync(c->h_ring[t.ring], c->d_ring[t.ring], (size_t)count * sizeof(RawFrame), cudaMemcpyDeviceToHost, c->s_d2h));
+	if (c->decode_stats)           /* the submit's demod is done (ev.c follows it): its counters travel with its frames */
+		CU(cudaMemcpyAsync(c->h_evcnt[t.ring], c->d_evcnt[t.ring], c->dstats.size() * EV_COUNT * sizeof(unsigned),
+		                   cudaMemcpyDeviceToHost, c->s_d2h));
 	CU(cudaEventRecord(c->ev_ring_read[t.ring], c->s_d2h));
 	c->ring_read_pending[t.ring] = true;
 	{
@@ -966,8 +1030,12 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		c->ring_read_pending[b] = false;
 	}
 	CU(cudaMemsetAsync(c->d_ctl[b], 0, sizeof(RingCtl), c->s_dem));
+	if (c->decode_stats) CU(cudaMemsetAsync(c->d_evcnt[b], 0, c->dstats.size() * EV_COUNT * sizeof(unsigned), c->s_dem));
 	CU(cudaEventRecord(t.ev.b2, c->s_dem));
-	int r = launch_demod(c->d_state, dmbuf, nsamp, c->cfg.nch, c->cfg.nstreams, c->d_ring[b], c->d_ctl[b], c->ring_cap, c->demod_lanes, c->s_dem);
+	int r = c->decode_stats ? launch_demod_stats(c->d_state, dmbuf, nsamp, c->cfg.nch, c->cfg.nstreams, c->d_ring[b], c->d_ctl[b],
+	                                             c->ring_cap, c->demod_lanes, c->d_evcnt[b], c->s_dem)
+	                        : launch_demod(c->d_state, dmbuf, nsamp, c->cfg.nch, c->cfg.nstreams, c->d_ring[b], c->d_ctl[b], c->ring_cap,
+	                                       c->demod_lanes, c->s_dem);
 	if (r) return fail(ACB_ERR_CUDA, "demod launch: %s", cudaGetErrorString((cudaError_t)r));
 	c->stats.kernel_launches++;
 	c->stats.demod_launches++;
@@ -976,7 +1044,8 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 	/* block FEC on the frames this submit appended (blk_thread's job, acars.c:93-215), in place — on its own stream:
 	 * it touches this submit's ring only, and the next demod need not wait behind it */
 	CU(cudaStreamWaitEvent(c->s_fec, c->ev_k2_done[b], 0));
-	r = launch_block_fec(c->d_ring[b], c->d_ctl[b], c->ring_cap, c->s_fec);
+	r = c->decode_stats ? launch_block_fec_stats(c->d_ring[b], c->d_ctl[b], c->ring_cap, c->s_fec)
+	                    : launch_block_fec(c->d_ring[b], c->d_ctl[b], c->ring_cap, c->s_fec);
 	if (r) return fail(ACB_ERR_CUDA, "block FEC launch: %s", cudaGetErrorString((cudaError_t)r));
 	c->stats.kernel_launches++;
 	CU(cudaMemcpyAsync(c->h_ctl[b], c->d_ctl[b], sizeof(RingCtl), cudaMemcpyDeviceToHost, c->s_fec));
@@ -1498,5 +1567,16 @@ extern "C" int acb_get_stats(acb_ctx_t *c, acb_stats_t *out, int reset)
 	std::lock_guard<std::mutex> lk(c->mtx);
 	*out = c->stats;
 	if (reset) memset(&c->stats, 0, sizeof(c->stats));
+	return ACB_OK;
+}
+
+extern "C" int acb_get_decode_stats(acb_ctx_t *c, acb_decode_stats_t *out, size_t n, int reset)
+{
+	if (!c || !out) return fail(ACB_ERR_ARG, "null argument");
+	if (!c->decode_stats) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_DECODE_STATS");
+	if (n < c->dstats.size()) return fail(ACB_ERR_ARG, "n=%zu < nstreams*nch=%zu", n, c->dstats.size());
+	std::lock_guard<std::mutex> lk(c->dstats_mtx);
+	memcpy(out, c->dstats.data(), c->dstats.size() * sizeof(acb_decode_stats_t));
+	if (reset) memset(c->dstats.data(), 0, c->dstats.size() * sizeof(acb_decode_stats_t));
 	return ACB_OK;
 }

@@ -14,6 +14,12 @@
  *   bool frame_begin();   // SOH seen: claim storage / note the time; false = no storage
  *   void frame_emit();    // frame complete: hand over (level is computed from lvlsum/bitcount)
  *
+ * and optionally
+ *
+ *   void event(int e);    // a FrameEvent below occurred (the decode statistics, ACB_FLAG_DECODE_STATS)
+ *
+ * An accessor without event() gets nothing: the calls compile away, so its code is what it was before the hook.
+ *
  * Integer-only apart from zeroing two doubles, so host and device agree trivially.
  */
 #ifndef ACB_FRAME_SM_H
@@ -33,6 +39,24 @@ constexpr unsigned char C_SYN = 0x16, C_NSYN = 0xE9, C_SOH = 0x01, C_STX = 0x02;
 constexpr unsigned char C_ETX = 0x83, C_ETB = 0x97, C_DLE = 0x7f;               /* acars.c:22-27 */
 constexpr int MAX_PARITY_ERR = 3;                                               /* acars.c:92 */
 
+/* The frame synchroniser's events (acb_decode_stats_t).  The first six are raised here; EV_SHORT and EV_LOST are the
+ * accessor's own, from where its frame_emit put the frame (a block under 13 bytes, acars.c:124-129; a full device ring). */
+enum FrameEvent {
+	EV_PREAMBLE = 0,       /* two SYN seen, waiting for SOH (acars.c:267-271) */
+	EV_STARTED,            /* SOH accepted, a block is assembled (acars.c:281-298) */
+	EV_TXT_PARITY,         /* block abandoned: too many parity errors (acars.c:307-317) */
+	EV_TXT_LONG,           /* block abandoned: over 240 bytes (acars.c:334-338) */
+	EV_TXT_MISSED_END,     /* DLE after 20 bytes, emitted anyway (acars.c:324-332) */
+	EV_EMITTED,            /* handed to the block FEC (acars.c:350-366) */
+	EV_SHORT,              /* emitted, shorter than 13 bytes */
+	EV_LOST,               /* emitted, found the device ring full */
+	EV_COUNT
+};
+
+template <class A> ACB_HD auto frame_event_(A &a, int e, int) -> decltype(a.event(e), void()) { a.event(e); }
+template <class A> ACB_HD void frame_event_(A &, int, long) {}
+template <class A> ACB_HD void frame_event(A &a, int e) { frame_event_(a, e, 0); }
+
 /* numbits[c] & 1 (syndrom.h:4-13): odd number of ones = parity ok */
 ACB_HD bool parity_ok(unsigned char c)
 {
@@ -51,6 +75,7 @@ template <class A> ACB_HD void frame_resync(A &a)
 
 template <class A> ACB_HD void frame_finish(A &a)
 {
+	frame_event(a, EV_EMITTED);
 	a.frame_emit();                         /* acars.c:350-366 */
 	a.state() = F_END;
 	a.nbits() = 8;
@@ -73,12 +98,13 @@ template <class A> ACB_HD void frame_byte(A &a, unsigned char r)
 	}
 	switch (a.state()) {
 	case F_SYN2:
-		if (r == C_SYN) { a.state() = F_SOH1; a.nbits() = 8; return; }
+		if (r == C_SYN) { frame_event(a, EV_PREAMBLE); a.state() = F_SOH1; a.nbits() = 8; return; }
 		if (r == C_NSYN) { a.msk_s() ^= 2u; a.nbits() = 8; return; }
 		frame_resync(a);
 		return;
 	case F_SOH1:
 		if (r != C_SOH || !a.frame_begin()) { frame_resync(a); return; }
+		frame_event(a, EV_STARTED);
 		a.state() = F_TXT;
 		a.blk_len() = 0;
 		a.blk_err() = 0;
@@ -91,10 +117,11 @@ template <class A> ACB_HD void frame_byte(A &a, unsigned char r)
 		a.txt_put(n, r);
 		a.blk_len() = ++n;
 		if (!parity_ok(r)) {
-			if (++a.blk_err() > MAX_PARITY_ERR + 1) { frame_resync(a); return; }
+			if (++a.blk_err() > MAX_PARITY_ERR + 1) { frame_event(a, EV_TXT_PARITY); frame_resync(a); return; }
 		}
 		if (r == C_ETX || r == C_ETB) { a.state() = F_CRC1; a.nbits() = 8; return; }
 		if (n > 20 && r == C_DLE) {         /* end of text was missed: the BCS is already in txt */
+			frame_event(a, EV_TXT_MISSED_END);
 			n -= 3;
 			a.blk_len() = n;
 			a.crc_put(0, a.txt_get(n));
@@ -102,7 +129,7 @@ template <class A> ACB_HD void frame_byte(A &a, unsigned char r)
 			frame_finish(a);
 			return;
 		}
-		if (n > 240) { frame_resync(a); return; }
+		if (n > 240) { frame_event(a, EV_TXT_LONG); frame_resync(a); return; }
 		a.nbits() = 8;
 		return;
 	}

@@ -2633,18 +2633,18 @@ int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride
  * ---------------------------------------------------------------------------------------- */
 
 /* acars.c:350-366: queue the finished block.  lvl = 10*log10(lvlsum/bitcount) is left to the host
- * (glibc log10) so the float matches the reference bit for bit.  Out of line and by value: it
- * runs once per frame, and keeping it away from the loop keeps the loop's state in registers. */
-static __device__ __noinline__ void emit_frame(const ChainState *st, RawFrame *ring, RingCtl *ctl, unsigned cap,
-                                               int stream, int chn, int len, int err, double lvlsum, int bitcount,
-                                               unsigned long long pos, unsigned long long soh_pos)
+ * (glibc log10) so the float matches the reference bit for bit.  Returns where the frame went: EV_SHORT, EV_LOST, or
+ * -1 = into the ring. */
+static __device__ __forceinline__ int emit_frame_at(const ChainState *st, RawFrame *ring, RingCtl *ctl, unsigned cap,
+                                                    int stream, int chn, int len, int err, double lvlsum, int bitcount,
+                                                    unsigned long long pos, unsigned long long soh_pos)
 {
 	/* blk_thread drops blocks shorter than 13 bytes unseen (acars.c:124-129): they never take a slot, so a
 	 * ring sized for the shortest deliverable frame (19 bytes on air = 792 samples) cannot be overrun by a
 	 * transmitter sending degenerate frames; the host adds the count to raw_frames / fec_dropped */
-	if (len < 13) { atomicAdd(&ctl->short_frames, 1u); return; }
+	if (len < 13) { atomicAdd(&ctl->short_frames, 1u); return EV_SHORT; }
 	const unsigned slot = atomicAdd(&ctl->count, 1u);
-	if (slot >= cap) return;                       /* overflow: counted by the host (frames_lost), decoding goes on */
+	if (slot >= cap) return EV_LOST;               /* overflow: counted by the host (frames_lost), decoding goes on */
 	RawFrame *f = ring + slot;
 	f->stream = stream; f->chn = chn;
 	f->len = len; f->err = err;
@@ -2655,6 +2655,24 @@ static __device__ __noinline__ void emit_frame(const ChainState *st, RawFrame *r
 	const uint2 *src = reinterpret_cast<const uint2 *>(st->txt);
 	uint2 *dst = reinterpret_cast<uint2 *>(f->txt);
 	for (int i = 0; i < TXTCAP / 8; i++) dst[i] = src[i];
+	return -1;
+}
+
+/* Out of line and by value: it runs once per frame, and keeping it away from the loop keeps the loop's state in
+ * registers. */
+static __device__ __noinline__ void emit_frame(const ChainState *st, RawFrame *ring, RingCtl *ctl, unsigned cap,
+                                               int stream, int chn, int len, int err, double lvlsum, int bitcount,
+                                               unsigned long long pos, unsigned long long soh_pos)
+{
+	emit_frame_at(st, ring, ctl, cap, stream, chn, len, err, lvlsum, bitcount, pos, soh_pos);
+}
+
+/* the counting kernels' form: the same, and where the frame went */
+static __device__ __noinline__ int emit_frame_counted(const ChainState *st, RawFrame *ring, RingCtl *ctl, unsigned cap,
+                                                      int stream, int chn, int len, int err, double lvlsum, int bitcount,
+                                                      unsigned long long pos, unsigned long long soh_pos)
+{
+	return emit_frame_at(st, ring, ctl, cap, stream, chn, len, err, lvlsum, bitcount, pos, soh_pos);
 }
 
 /* accessor for frame_sm.h: state in registers, text in the chain's HBM record */
@@ -2685,6 +2703,22 @@ struct DevFrameAcc {
 	__device__ __forceinline__ void frame_emit()
 	{
 		if (leader) emit_frame(st, ring, ctl, cap, stream, chn, r.blk_len, r.blk_err, r.lvlsum, r.bitcount, bit_pos(), r.soh_pos);
+	}
+};
+
+/* The counting kernels' accessor (ACB_FLAG_DECODE_STATS): DevFrameAcc plus the event hook.  Only the leader lane writes,
+ * only on the rare events of frame_sm.h (no SYN-hunting bit raises one), into its chain's counters of this submit; no
+ * other lane shares them, so plain increments do. */
+struct DevFrameAccStats : DevFrameAcc {
+	unsigned *cnt;           /* EV_COUNT counters of this chain */
+
+	__device__ __forceinline__ void event(int e) { if (leader) cnt[e]++; }
+	__device__ __forceinline__ void frame_emit()
+	{
+		if (!leader) return;
+		const int where = emit_frame_counted(st, ring, ctl, cap, stream, chn, r.blk_len, r.blk_err, r.lvlsum, r.bitcount, bit_pos(),
+		                                     r.soh_pos);
+		if (where >= 0) cnt[where]++;
 	}
 };
 
@@ -2977,13 +3011,14 @@ int upload_matched_filter(const float *h, cudaStream_t stream)
 	return (int)cudaStreamSynchronize(stream);
 }
 
-template <int L, bool F2F, bool PIN, int MINB = 1>     /* MINB = 0: no occupancy request */
-__global__ void __launch_bounds__(32, MINB)
-k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsamp, int nch, int nstreams,
-         int wps, RawFrame *__restrict__ ring, RingCtl *__restrict__ ctl, unsigned cap)
+/* K2's body, shared by k_demod2 and its counting form k_demod2_stats (STATS: the frame synchroniser's events go to
+ * counts[chain * EV_COUNT + e]; k_demod2 passes none and never sees the hook) */
+template <int L, bool F2F, bool PIN, bool STATS>
+__device__ __forceinline__ void demod2_body(DemodShared<32 / L> &sm, ChainState *__restrict__ states, const float *__restrict__ dm,
+                                            int nsamp, int nch, int nstreams, RawFrame *__restrict__ ring,
+                                            RingCtl *__restrict__ ctl, unsigned cap, unsigned *__restrict__ counts)
 {
 	constexpr int CPW = 32 / L;                  /* channels per warp */
-	__shared__ DemodShared<CPW> sm;
 	const int lane = threadIdx.x;
 	for (int i = lane; i < 64; i += 32) {
 		sm.tcos[i].x = g_sc_cos[i].x; sm.tcos[i].y = g_sc_cos[i].y;
@@ -3000,7 +3035,6 @@ k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsam
 	const long long g = valid ? g_raw : nchain - 1;
 	const int s = (int)(g / nch), ch = (int)(g - (long long)s * nch);
 	const bool leader = valid && sub == 0;
-	(void)wps;
 
 	ChainState *st = states + (size_t)s * nch + ch;
 	DemodRegs r;
@@ -3015,8 +3049,13 @@ k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsam
 	}
 	__syncwarp();
 
-	DevFrameAcc acc{ r, st, ring, ctl, cap, s, ch, leader, true };
-	demod_run<L, F2F, PIN, WarpEnv>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, nsamp, sub, grp, acc);
+	if constexpr (STATS) {
+		DevFrameAccStats acc{ { r, st, ring, ctl, cap, s, ch, leader, true }, counts + (size_t)g * EV_COUNT };
+		demod_run<L, F2F, PIN, WarpEnv>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, nsamp, sub, grp, acc);
+	} else {
+		DevFrameAcc acc{ r, st, ring, ctl, cap, s, ch, leader, true };
+		demod_run<L, F2F, PIN, WarpEnv>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, nsamp, sub, grp, acc);
+	}
 
 	if (!leader) return;
 	st->phi = r.phi; st->df = r.df; st->lvlsum = r.lvlsum; st->clk = r.clk; st->bitcount = r.bitcount;
@@ -3024,6 +3063,26 @@ k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsam
 	st->blk_len = r.blk_len; st->blk_err = r.blk_err; st->pos = r.pos; st->soh_pos = r.soh_pos;
 #pragma unroll
 	for (int k = 0; k < FLEN; k++) { st->inb_re[k] = sm.ring[k][grp].x; st->inb_im[k] = sm.ring[k][grp].y; }
+}
+
+template <int L, bool F2F, bool PIN, int MINB = 1>     /* MINB = 0: no occupancy request */
+__global__ void __launch_bounds__(32, MINB)
+k_demod2(ChainState *__restrict__ states, const float *__restrict__ dm, int nsamp, int nch, int nstreams,
+         int wps, RawFrame *__restrict__ ring, RingCtl *__restrict__ ctl, unsigned cap)
+{
+	__shared__ DemodShared<32 / L> sm;
+	(void)wps;
+	demod2_body<L, F2F, PIN, false>(sm, states, dm, nsamp, nch, nstreams, ring, ctl, cap, nullptr);
+}
+
+/* the counting form (ACB_FLAG_DECODE_STATS): the same launch geometry, launch bounds and shared memory */
+template <int L, bool F2F, bool PIN, int MINB = 1>
+__global__ void __launch_bounds__(32, MINB)
+k_demod2_stats(ChainState *__restrict__ states, const float *__restrict__ dm, int nsamp, int nch, int nstreams,
+               RawFrame *__restrict__ ring, RingCtl *__restrict__ ctl, unsigned cap, unsigned *__restrict__ counts)
+{
+	__shared__ DemodShared<32 / L> sm;
+	demod2_body<L, F2F, PIN, true>(sm, states, dm, nsamp, nch, nstreams, ring, ctl, cap, counts);
 }
 
 /* SM count and shared memory per SM of the current device, asked per launch: contexts of one process may sit on
@@ -3060,9 +3119,9 @@ constexpr int DEMOD_SMEM_BESIDE = 3 * (4096 + DEMOD_SMEM_RESERVED);   /* three k
 constexpr int DEMOD_MAX_WARPS_PER_SM = 16;
 constexpr int DEMOD_MIN_WARPS_SHARING = 4;                      /* per SM: below, K2 is the step and keeps the largest carve-out */
 
-template <int LANES, bool F2F, bool PIN, int MINB = 1>
+template <int LANES, bool F2F, bool PIN, int MINB = 1, bool STATS = false>
 static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                          RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
+                          RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
 {
 	constexpr int CPW = 32 / LANES;
 	const int wps = (nch + CPW - 1) / CPW;
@@ -3074,6 +3133,12 @@ static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, i
 	const long long need = per_sm * ((long long)sizeof(DemodShared<CPW>) + DEMOD_SMEM_RESERVED) + DEMOD_SMEM_BESIDE;
 	const int carve = per_sm < DEMOD_MIN_WARPS_SHARING ? (int)cudaSharedmemCarveoutMaxShared
 	                                                   : (int)std::min<long long>(100, (need * 100 + smem_per_sm - 1) / smem_per_sm);
+	if constexpr (STATS) {
+		cudaError_t e = cudaFuncSetAttribute(k_demod2_stats<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
+		if (e != cudaSuccess) return (int)e;
+		k_demod2_stats<LANES, F2F, PIN, MINB><<<grid, 32, 0, stream>>>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, counts);
+		return (int)cudaGetLastError();
+	}
 	cudaError_t e = cudaFuncSetAttribute(k_demod2<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
 	if (e != cudaSuccess) return (int)e;
 	k_demod2<LANES, F2F, PIN, MINB><<<grid, 32, 0, stream>>>(st, dm, nsamp, nch, nstreams, wps, ring, ctl, cap);
@@ -3084,15 +3149,15 @@ static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, i
  * (__launch_bounds__(32, 1)), ptxas spends more registers on a wider schedule: fewer instructions where the kernel is
  * latency bound, but fewer warps per SM where it is not.  So: the wide schedule while there are at most 8 warps per SM,
  * the lean one beyond. */
-template <int LANES, bool F2F>
+template <int LANES, bool F2F, bool STATS = false>
 static int launch_demod_pinned(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                               RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
+                               RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
 {
 	int sm_count, smem_per_sm;
 	demod_sm_limits(sm_count, smem_per_sm);
 	const long long warps = ((long long)nstreams * nch * LANES + 31) / 32;
-	return warps <= 8LL * sm_count ? launch_demod_t<LANES, F2F, true, 1>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream)
-	                               : launch_demod_t<LANES, F2F, true, 0>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream);
+	return warps <= 8LL * sm_count ? launch_demod_t<LANES, F2F, true, 1, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts)
+	                               : launch_demod_t<LANES, F2F, true, 0, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts);
 }
 
 /* The one-lane form in two register budgets.  Left alone ptxas takes 128 registers per thread; of those CTAs six fit
@@ -3103,15 +3168,16 @@ static int launch_demod_pinned(ChainState *st, const float *dm, int nsamp, int n
 constexpr int DEMOD_MINB_96REG = 20;
 constexpr int DEMOD_WARPS_PER_K1_CTA = 6;
 
+template <bool STATS = false>
 static int launch_demod_one_lane(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                                 RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream)
+                                 RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
 {
 	int sm_count, smem_per_sm;
 	demod_sm_limits(sm_count, smem_per_sm);
 	const long long warps = ((long long)nstreams * nch + 31) / 32;
 	return warps <= (long long)DEMOD_WARPS_PER_K1_CTA * sm_count
-	           ? launch_demod_t<1, false, false, 1>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream)
-	           : launch_demod_t<1, false, false, DEMOD_MINB_96REG>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream);
+	           ? launch_demod_t<1, false, false, 1, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts)
+	           : launch_demod_t<1, false, false, DEMOD_MINB_96REG, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts);
 }
 
 template <int LANES>
@@ -3153,7 +3219,7 @@ int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstrea
 	case -4: return launch_demod_v1<4>(ACB_DEMOD_ARGS);
 	case 8: return launch_demod_pinned<8, false>(ACB_DEMOD_ARGS);
 	case 2: return launch_demod_pinned<2, false>(ACB_DEMOD_ARGS);
-	case 1: return launch_demod_one_lane(ACB_DEMOD_ARGS);
+	case 1: return launch_demod_one_lane<>(ACB_DEMOD_ARGS);
 	case 17: return launch_demod_t<1, true, false>(ACB_DEMOD_ARGS);          /* F2F bit clock at one lane */
 	case 24: return launch_demod_pinned<8, true>(ACB_DEMOD_ARGS);
 	case 20: return launch_demod_pinned<4, true>(ACB_DEMOD_ARGS);
@@ -3162,6 +3228,22 @@ int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstrea
 	case 34: return launch_demod_t<2, false, false>(ACB_DEMOD_ARGS);
 	case 33: return launch_demod_t<1, false, true>(ACB_DEMOD_ARGS);
 	default: return launch_demod_pinned<4, false>(ACB_DEMOD_ARGS);
+	}
+#undef ACB_DEMOD_ARGS
+}
+
+/* the counting forms of the default widths (what launch_demod runs for lanes 1, 2, 4, 8), each in the same register
+ * budgets and under the same carve-out rules */
+int launch_demod_stats(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
+                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes, unsigned *counts, cudaStream_t stream)
+{
+#define ACB_DEMOD_ARGS st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts
+	switch (lanes) {
+	case 8: return launch_demod_pinned<8, false, true>(ACB_DEMOD_ARGS);
+	case 4: return launch_demod_pinned<4, false, true>(ACB_DEMOD_ARGS);
+	case 2: return launch_demod_pinned<2, false, true>(ACB_DEMOD_ARGS);
+	case 1: return launch_demod_one_lane<true>(ACB_DEMOD_ARGS);
+	default: return (int)cudaErrorInvalidValue;
 	}
 #undef ACB_DEMOD_ARGS
 }
@@ -3190,11 +3272,12 @@ __device__ __forceinline__ bool fec_crc_bytes_hit(const unsigned short *syn, uns
 	return hit;
 }
 
-__global__ void __launch_bounds__(128)
-k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsigned cap)
+/* K3's body, shared by k_block_fec and its counting form k_block_fec_stats (STATS: each frame's FEC_WHY_* also goes to
+ * RawFrame::pad1[0], following blk_thread's control flow) */
+template <bool STATS>
+__device__ __forceinline__ void block_fec_body(unsigned short *s_crc, unsigned short *s_syn, RawFrame *__restrict__ ring,
+                                               const RingCtl *__restrict__ ctl, unsigned cap)
 {
-	__shared__ unsigned short s_crc[256];
-	__shared__ unsigned short s_syn[8 * FEC_SYN_BYTES];
 	/* the grid is sized for the busiest step (one thread per frame up to 4 * SMs * 128 frames, 67 584 on a 132-SM H100,
 	 * then a stride loop; tests/test_gpu_scale.py runs more than two passes); CTAs
 	 * with no frame leave before building the tables */
@@ -3220,8 +3303,9 @@ k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsign
 		unsigned char *txt = fr->txt;
 		const int len = fr->len;
 		int status = 2;
+		unsigned why = 0;
 		do {
-			if (len < 13 || len > 250) break;                                 /* acars.c:124-129 */
+			if (len < 13 || len > 250) { why = FEC_WHY_SHORT; break; }        /* acars.c:124-129 */
 			txt[12] = (unsigned char)((txt[12] & 0x83u) | 0x02u);             /* force STX/ETX, acars.c:132-133 */
 			int bad[3], nbad = 0;
 			unsigned crc = 0;
@@ -3230,10 +3314,11 @@ k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsign
 				if ((__popc(c) & 1) == 0) { if (nbad < 3) bad[nbad] = i; nbad++; }
 				crc = fec_crc_step(s_crc, crc, c);
 			}
-			if (nbad > 3) break;                                              /* acars.c:145-152 */
+			if (nbad > 3) { why = FEC_WHY_PARITY_EXCESS; break; }             /* acars.c:145-152 */
 			crc = fec_crc_step(s_crc, crc, fr->crc[0]);
 			crc = fec_crc_step(s_crc, crc, fr->crc[1]);
 			fr->err = nbad;
+			why = (nbad ? FEC_WHY_PARITY : 0u) | (crc ? FEC_WHY_CRC : 0u);      /* acars.c:153-155, 166-167 */
 			bool ok = true;
 			if (nbad) {
 				/* fixprerr, depth first in the reference's order: bit of the first bad byte outermost */
@@ -3275,7 +3360,8 @@ k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsign
 							}
 				}
 			}
-			if (!ok) break;
+			if (!ok) { why |= FEC_WHY_UNFIXABLE; break; }                     /* acars.c:171-175, 183-187 */
+			if (nbad || crc) why |= FEC_WHY_FIXED;                            /* acars.c:177-178, 189-190 */
 			int still = 0;                                                    /* acars.c:194-207 */
 			for (int i = 0; i < len; i++) {
 				const unsigned c = txt[i];
@@ -3283,9 +3369,27 @@ k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsign
 				txt[i] = (unsigned char)(c & 0x7fu);
 			}
 			status = still ? 2 : 1;
+			if (still) why |= FEC_WHY_PARITY_PROBLEM;
 		} while (0);
 		fr->pad0 = status;
+		if (STATS) fr->pad1[0] = (unsigned char)why;
 	}
+}
+
+__global__ void __launch_bounds__(128)
+k_block_fec(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsigned cap)
+{
+	__shared__ unsigned short s_crc[256];
+	__shared__ unsigned short s_syn[8 * FEC_SYN_BYTES];
+	block_fec_body<false>(s_crc, s_syn, ring, ctl, cap);
+}
+
+__global__ void __launch_bounds__(128)
+k_block_fec_stats(RawFrame *__restrict__ ring, const RingCtl *__restrict__ ctl, unsigned cap)
+{
+	__shared__ unsigned short s_crc[256];
+	__shared__ unsigned short s_syn[8 * FEC_SYN_BYTES];
+	block_fec_body<true>(s_crc, s_syn, ring, ctl, cap);
 }
 
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, cudaStream_t stream)
@@ -3294,6 +3398,15 @@ int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, cudaStrea
 	if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0)
 		sm_count = 132;
 	k_block_fec<<<4 * sm_count, 128, 0, stream>>>(ring, ctl, cap);
+	return (int)cudaGetLastError();
+}
+
+int launch_block_fec_stats(RawFrame *ring, const RingCtl *ctl, unsigned cap, cudaStream_t stream)
+{
+	int dev = 0, sm_count = 0;
+	if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0)
+		sm_count = 132;
+	k_block_fec_stats<<<4 * sm_count, 128, 0, stream>>>(ring, ctl, cap);
 	return (int)cudaGetLastError();
 }
 

@@ -312,3 +312,19 @@ extern "C" int acb_multi_set_state(acb_multi_t *m, int stream, int chn, const ac
 	Part *p = m ? find(m, stream, chn) : nullptr;
 	return p ? acb_set_state(p->ctx, stream - p->s0, chn - p->c0, in) : ACB_ERR_ARG;
 }
+
+/* each part's table, placed at the global indices of its chains */
+extern "C" int acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *out, size_t n, int reset)
+{
+	if (!m || !out) return fail(ACB_ERR_ARG, "null argument");
+	const int nch = m->cfg.nch;
+	if (n < (size_t)m->cfg.nstreams * nch) return fail(ACB_ERR_ARG, "n=%zu < nstreams*nch", n);
+	std::vector<acb_decode_stats_t> part;
+	for (auto &p : m->parts) {
+		part.resize((size_t)p.ns * p.nc);
+		if (int r = acb_get_decode_stats(p.ctx, part.data(), part.size(), reset)) return r;
+		for (int s = 0; s < p.ns; s++)
+			for (int c = 0; c < p.nc; c++) out[(size_t)(p.s0 + s) * nch + p.c0 + c] = part[(size_t)s * p.nc + c];
+	}
+	return ACB_OK;
+}

@@ -146,6 +146,13 @@ typedef struct {
                                          ACB_FLAG_FAST_WIDEBAND alone selects nothing on a real context. */
 #define ACB_FLAG_REAL_INPUT 2         /* Airspy front-end (air.c): float32 REAL samples at IF = rate/4,
                                          rate = K*12500; use acb_set_plan_air / acb_submit_real_host */
+#define ACB_FLAG_DECODE_STATS 256     /* keep per-chain decode statistics (acb_decode_stats_t, acb_get_decode_stats): why
+                                         frames were lost, counted where the reference's -v output prints a line.  The
+                                         demodulator and the block FEC run their counting forms (same arithmetic, same
+                                         launch rules); messages, envelope and chain states are unchanged.  Any input kind
+                                         and channelizer form.  With this flag, ACB_DEMOD_LANES values other than 1, 2, 4 and
+                                         8 are ignored and the picked default width runs (the other kernel forms have no
+                                         counting form).  Without it acb_get_decode_stats returns ACB_ERR_ARG. */
 
 /* One decoded block, after parity/CRC repair: msgblk_t (acarsdec.h:48-57) without the queue
  * link, plus where it came from.  `txt` is parity-stripped (acars.c:200). */
@@ -425,6 +432,40 @@ typedef struct {
 } acb_stats_t;
 int acb_get_stats(acb_ctx_t *ctx, acb_stats_t *out, int reset);
 
+/* Per-chain decode statistics (ACB_FLAG_DECODE_STATS): for one (stream, channel), how many times each event of the
+ * frame synchroniser (decodeAcars) and of the block FEC (blk_thread) occurred — the reference's -v output as counts
+ * (one count per kind of line and channel; the log itself is not produced).  Each field names its event:
+ *   preamble            two SYN seen, waiting for SOH (acars.c:267-271)
+ *   started             SOH accepted, a block is being assembled (acars.c:281-298)
+ *   txt_parity          block abandoned: more than MAXPERR+1 bad bytes (acars.c:307-317, "too many parity errors")
+ *   txt_long            block abandoned: over 240 bytes (acars.c:334-338, "too long")
+ *   txt_missed_end      DLE after 20 bytes, emitted anyway (acars.c:324-332, "miss txt end")
+ *   emitted             handed to the block FEC (acars.c:350-366, "put message")
+ *   fec_short           shorter than 13 bytes (acars.c:124-129, "too short")
+ *   fec_parity_excess   more than MAXPERR parity errors (acars.c:145-152, "too many parity errors: %d")
+ *   fec_parity          1..MAXPERR parity errors (acars.c:153-155, "parity error(s)")
+ *   fec_crc             CRC non-zero (acars.c:166-167, "crc error")
+ *   fec_fixed           repaired (acars.c:177-178, 189-190, "errors fixed")
+ *   fec_unfixable       not repairable (acars.c:172-173, 184-185, "not able to fix errors")
+ *   fec_parity_problem  the final parity re-check failed (acars.c:202-206, "parity check problem")
+ *   delivered           queued for acb_drain (outputmsg, acars.c:209)
+ *   lost                found the device ring full (this chain's part of acb_stats_t.frames_lost)
+ * Per chain, at any time:
+ *   emitted   = fec_short + fec_parity_excess + fec_unfixable + fec_parity_problem + delivered + lost
+ *   started   = emitted + txt_parity + txt_long + (1 while a block is open: Acarsstate TXT, CRC1 or CRC2)
+ *   delivered = the messages acb_drain returns for the chain
+ * (the second holds for chain states the context produced itself; acb_set_state can open or close a block). */
+typedef struct {
+	uint64_t preamble, started, txt_parity, txt_long, txt_missed_end, emitted;
+	uint64_t fec_short, fec_parity_excess, fec_parity, fec_crc, fec_fixed, fec_unfixable, fec_parity_problem;
+	uint64_t delivered, lost;
+} acb_decode_stats_t;
+/* Fills out[s*nch + c] for every chain; n >= nstreams*nch.  The counts cover exactly the submits acb_collect / acb_sync
+ * have covered (the ones whose messages acb_drain returns); a submit abandoned by acb_reset contributes nothing, and
+ * acb_reset clears the counts along with the undrained messages.  reset != 0 clears them after reading.  ACB_ERR_ARG
+ * without ACB_FLAG_DECODE_STATS. */
+int acb_get_decode_stats(acb_ctx_t *ctx, acb_decode_stats_t *out, size_t n, int reset);
+
 /* ---- one process, several GPUs (the C host's way to a whole node; SURVEY.md §8e) ----
  *
  * acb_multi_* fronts one context per device.  Two ways to cut the work, neither with any device-to-device
@@ -471,6 +512,8 @@ int  acb_multi_sync(acb_multi_t *m);
 int  acb_multi_drain(acb_multi_t *m, acb_msg_t *out, int max);
 int  acb_multi_get_state(acb_multi_t *m, int stream, int chn, acb_chan_state_t *out);
 int  acb_multi_set_state(acb_multi_t *m, int stream, int chn, const acb_chan_state_t *in);
+/* acb_get_decode_stats over the parts, indexed by global stream and channel: out[s*nch + c], n >= nstreams*nch */
+int  acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *out, size_t n, int reset);
 
 /* Block FEC on one frame in place on the HOST (acars.c:123-207): 1 = deliver, 0 = drop.  The
  * processing path runs the same repair on the device (k_block_fec, one thread per frame, right
