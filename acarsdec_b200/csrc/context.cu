@@ -72,6 +72,24 @@ struct EvTriple { cudaEvent_t a, b, b2, c; bool chan; };   /* a..b = K1 on s_com
  * behind that of N+1 and both kernels run back to back on their streams. */
 constexpr int NPIPE = 3;
 
+/* K1, the channelizer: the form a context runs, chosen once by chan_form() and tried in this order
+ *
+ *   input       condition                                                      form
+ *   u8 / CS16   ACB_FLAG_FAST_CHANNELIZER, taps == K, K in {160, 192}          CHAN_DFT       k_channelize_dft(1)
+ *               ACB_FLAG_FAST_FILTER, taps > K, K in {160, 192}                CHAN_OVL_FAST  k_channelize_ovl_fast
+ *               ACB_FLAG_FAST_WIDEBAND, taps >= K, K % 8 == 0                  CHAN_WB        k_channelize_wb
+ *               K % 8 != 0 (u8), K % 4 != 0 (CS16)                             CHAN_GENERIC   k_channelize_generic(_ovl)
+ *               otherwise                                                      CHAN_EXACT     k_channelize_iq4
+ *   real        ACB_FLAG_FAST_CHANNELIZER, taps == K, channelize_rdft_supports  CHAN_RDFT      k_channelize_rdft
+ *               ACB_FLAG_FAST_FILTER_REAL, taps > K, channelize_rdft_supports  CHAN_OVL_RDFT  k_channelize_ovl_rdft
+ *               ACB_FLAG_FAST_WIDEBAND_REAL, taps >= K, K % 8 == 0             CHAN_WB_REAL   k_channelize_wb_real
+ *               K % 4 != 0                                                     CHAN_GENERIC   k_channelize_generic(_ovl)
+ *               otherwise                                                      CHAN_EXACT     k_channelize_real4
+ *
+ * A fast form (all but EXACT and GENERIC) runs only while every stream is planned on the 12.5 kHz raster (fast_ok); a
+ * submit runs EXACT otherwise. */
+enum ChanForm { CHAN_EXACT, CHAN_GENERIC, CHAN_DFT, CHAN_RDFT, CHAN_OVL_FAST, CHAN_OVL_RDFT, CHAN_WB, CHAN_WB_REAL };
+
 /* one submit in flight: which frame ring it appends to and how its frames are grouped */
 struct Ticket {
 	EvTriple ev;                                   /* a..b = channelizer, b..c = demod; c = done */
@@ -89,20 +107,14 @@ struct acb_ctx {
 	bool buf_used[2];
 	int next_buf;
 	float *d_wf;                 /* [stream][grp][taps_pad][8] float2 (c, d) */
-	bool fast;                   /* ACB_FLAG_FAST_CHANNELIZER and a shape k_channelize_dft takes */
-	bool fast_ovl;               /* taps > K and the polyphase form: ACB_FLAG_FAST_FILTER on u8 / CS16 with a K
-	                                k_channelize_ovl_fast takes, ACB_FLAG_FAST_FILTER_REAL on real input with a K
-	                                k_channelize_ovl_rdft takes */
-	bool wb;                     /* ACB_FLAG_FAST_WIDEBAND on u8 / CS16 (k_channelize_wb) or ACB_FLAG_FAST_WIDEBAND_REAL on
-	                                real input (k_channelize_wb_real), K % 8 == 0, taps >= K, and neither of the above
-	                                selects a narrow kernel */
-	float *d_wbE;                /* wb: the twiddle table(s) E of acb_wb_twiddles, 2K - 1 (Tr, Ti) each; CS16: one per variant */
-	int *d_wbmeta;               /* wb: [stream][channel tile][WB_META] residue-sorted slots (upload_wb_plan) */
-	float *d_p;                  /* fast_ovl, wb at taps > K: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
-	bool fold8;                  /* fast form: fold the row in half first (8-way split, K/8 MACs per channel) */
+	ChanForm form;
+	float *d_wbE;                /* WB*: the twiddle table(s) E of acb_wb_twiddles, 2K - 1 (Tr, Ti) each; CS16: one per variant */
+	int *d_wbmeta;               /* WB*: [stream][channel tile][WB_META] residue-sorted slots (upload_wb_plan) */
+	float *d_p;                  /* OVL_*, WB* at taps > K: the pre-sum weights fl(K*h), taps_pad floats, zeros in front */
+	bool fold8;                  /* DFT: fold the row in half first (8-way split, K/8 MACs per channel) */
 	int demod_lanes;             /* lanes per channel in k_demod: 8 for small contexts, else 4 */
-	float *d_tw;                 /* fast form: [stream][grp][8 ch][K/4] (Tr, Ti) twiddles */
-	unsigned *d_twmeta;          /* fast form: [stream][grp] residues k_c mod 4, 2 bits per channel slot */
+	float *d_tw;                 /* DFT, RDFT, OVL_*: [stream][grp][8 ch][K/4] (Tr, Ti) twiddles */
+	unsigned *d_twmeta;          /* DFT, RDFT, OVL_*: [stream][grp] residues k_c mod 4, 2 bits per channel slot */
 	std::vector<unsigned char> fast_ok;   /* per stream: planned on the 12.5 kHz raster (0 after acb_set_wf: caller's own table) */
 	float *d_dm[NPIPE];          /* [stream][nsamp][nch], one per submit in flight */
 	cudaEvent_t ev_k1_done[NPIPE], ev_dm_free[NPIPE], ev_k2_done[NPIPE], ev_ring_read[NPIPE];
@@ -142,7 +154,6 @@ struct acb_ctx {
 	cudaEvent_t mark[2], ev_join;
 	bool overflowed;
 	acb_stats_t stats;
-	bool use_generic;
 	int taps;                    /* FIR length per output row (<= ACB_MAXTAPS_PER_K * K) */
 	int taps_pad;                /* taps <= K: taps rounded up to whole 16-byte units of input (zero weights behind);
 	                                taps > K: K + hpad (zero weights in front) */
@@ -267,6 +278,22 @@ static int reset_states(acb_ctx *c)
 	return ACB_OK;
 }
 
+/* the table at ChanForm */
+static ChanForm chan_form(const acb_config_t *cfg, int in_kind, int taps)
+{
+	const int K = cfg->K, f = cfg->flags;
+	if (in_kind == IN_KIND_F32REAL) {
+		if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_rdft_supports(K)) return CHAN_RDFT;
+		if ((f & ACB_FLAG_FAST_FILTER_REAL) && taps > K && channelize_rdft_supports(K)) return CHAN_OVL_RDFT;
+		if ((f & ACB_FLAG_FAST_WIDEBAND_REAL) && taps >= K && K % 8 == 0) return CHAN_WB_REAL;
+		return K % 4 ? CHAN_GENERIC : CHAN_EXACT;
+	}
+	if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_dft_supports(K)) return CHAN_DFT;
+	if ((f & ACB_FLAG_FAST_FILTER) && taps > K && channelize_dft_supports(K)) return CHAN_OVL_FAST;
+	if ((f & ACB_FLAG_FAST_WIDEBAND) && taps >= K && K % 8 == 0) return CHAN_WB;
+	return K % (in_kind == IN_KIND_U8IQ ? 8 : 4) ? CHAN_GENERIC : CHAN_EXACT;
+}
+
 extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 {
 	if (!cfg || !out) return fail(ACB_ERR_ARG, "null argument");
@@ -293,8 +320,8 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->blk_bytes = (size_t)OUTBLK * cfg->K * 2;
 	c->in_kind = (cfg->flags & ACB_FLAG_REAL_INPUT) ? IN_KIND_F32REAL : (cfg->flags & ACB_FLAG_CS16_INPUT) ? IN_KIND_CS16IQ : IN_KIND_U8IQ;
 	c->real_input = c->in_kind != IN_KIND_U8IQ;
-	c->use_generic = c->real_input ? (cfg->K % 4) != 0 : (cfg->K % 8) != 0;
 	c->taps = cfg->taps ? cfg->taps : cfg->K;
+	c->form = chan_form(cfg, c->in_kind, c->taps);
 	{
 		const int per_unit = c->real_input ? 4 : 8;          /* taps per 16 bytes of input (4-byte vs 2-byte taps) */
 		c->hpad = 0;
@@ -308,7 +335,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 			c->hpad = (c->taps - cfg->K + per_unit - 1) / per_unit * per_unit;
 			c->taps_pad = cfg->K + c->hpad;
 		} else {
-			c->taps_pad = c->use_generic ? c->taps : (c->taps + per_unit - 1) / per_unit * per_unit;
+			c->taps_pad = c->form == CHAN_GENERIC ? c->taps : (c->taps + per_unit - 1) / per_unit * per_unit;
 			if (c->taps_pad > cfg->K) c->taps_pad = cfg->K;      /* K itself is a multiple of per_unit here */
 		}
 	}
@@ -386,13 +413,6 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	CU(cudaMalloc(&c->d_wf, wf_floats * sizeof(float)));
 	CU(cudaMemsetAsync(c->d_wf, 0, wf_floats * sizeof(float), c->s_copy));
 	CU(cudaStreamSynchronize(c->s_copy));
-	c->fast = (cfg->flags & ACB_FLAG_FAST_CHANNELIZER) && c->taps == cfg->K &&
-	          (c->in_kind == IN_KIND_F32REAL ? channelize_rdft_supports(cfg->K) : channelize_dft_supports(cfg->K));
-	c->fast_ovl = c->taps > cfg->K &&
-	              (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_FILTER_REAL) && channelize_rdft_supports(cfg->K)
-	                                             : (cfg->flags & ACB_FLAG_FAST_FILTER) && channelize_dft_supports(cfg->K));
-	c->wb = (c->in_kind == IN_KIND_F32REAL ? (cfg->flags & ACB_FLAG_FAST_WIDEBAND_REAL) : (cfg->flags & ACB_FLAG_FAST_WIDEBAND)) &&
-	        cfg->K % 8 == 0 && c->taps >= cfg->K && !c->fast && !c->fast_ovl;
 	c->d_wbE = nullptr;
 	c->d_wbmeta = nullptr;
 	c->d_p = nullptr;
@@ -414,11 +434,12 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 				c->demod_lanes = v;
 		}
 	}
-	if (c->fast || c->fast_ovl) {
+	const bool wb = c->form == CHAN_WB || c->form == CHAN_WB_REAL, ovl = c->form == CHAN_OVL_FAST || c->form == CHAN_OVL_RDFT;
+	if (ovl || c->form == CHAN_DFT || c->form == CHAN_RDFT) {
 		CU(cudaMalloc(&c->d_tw, (size_t)cfg->nstreams * c->ngrp * CH_GROUP * (cfg->K / 4) * 2 * sizeof(float)));
 		CU(cudaMalloc(&c->d_twmeta, (size_t)cfg->nstreams * c->ngrp * sizeof(unsigned)));
 	}
-	if (c->wb) {
+	if (wb) {
 		const int ntab = c->in_kind == IN_KIND_CS16IQ ? 2 : 1;
 		const size_t per = (size_t)(2 * cfg->K - 1) * 2;
 		std::vector<float> E(ntab * per);
@@ -429,7 +450,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		const size_t nct = (size_t)(cfg->nch + WB_CTILE - 1) / WB_CTILE;
 		CU(cudaMalloc(&c->d_wbmeta, (size_t)cfg->nstreams * nct * WB_META * sizeof(int)));
 	}
-	if (c->fast_ovl || (c->wb && c->hpad)) {
+	if (ovl || (wb && c->hpad)) {
 		/* the polyphase weights p[i] = fl(K * h[i]), laid out like the exact table (taps_pad entries, the hpad - H in front
 		 * zero): the same for every channel and stream; with the twiddles' 1/K the pre-sum's bin carries h[i] * scale */
 		std::vector<float> h(c->taps), p(c->taps_pad, 0.0f);
@@ -564,11 +585,9 @@ extern "C" int acb_set_wf(acb_ctx_t *c, int stream, const float *wf, int nch)
 	return ACB_OK;
 }
 
-/* fast form: group the per-channel twiddles and bin residues the way k_channelize_dft* reads them and upload them;
- * `ok` false (a channel off the raster) leaves the stream on the exact kernel */
-static int upload_fast_plan(acb_ctx *c, int stream, bool ok, const std::vector<int> &kbin, const std::vector<float> &tw1)
+/* DFT, RDFT, OVL_*: group the per-channel twiddles and bin residues the way the kernels read them and upload them */
+static int upload_fast_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, const std::vector<float> &tw1)
 {
-	if (!ok) return ACB_OK;
 	const int nch = c->cfg.nch, N2 = c->cfg.K / 4;
 	std::vector<float> tw((size_t)c->ngrp * CH_GROUP * N2 * 2, 0.0f);
 	std::vector<unsigned> meta(c->ngrp, 0u);
@@ -586,11 +605,9 @@ static int upload_fast_plan(acb_ctx *c, int stream, bool ok, const std::vector<i
 
 /* wideband form: per channel tile, the channel slots sorted by bin residue (k/2) mod 4 (real input: by the column the
  * real form reads, k mod 4 = 0, 2 or odd) and each class padded to whole groups of WB_CB (channel -1), so that every
- * thread of k_channelize_wb(_real) multiplies one Y' column; `etab` selects the twiddle table (CS16: the variant).  `ok`
- * false leaves the stream on the exact kernel. */
-static int upload_wb_plan(acb_ctx *c, int stream, bool ok, const std::vector<int> &kbin, int etab)
+ * thread of k_channelize_wb(_real) multiplies one Y' column; `etab` selects the twiddle table (CS16: the variant) */
+static int upload_wb_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, int etab)
 {
-	if (!ok) return ACB_OK;
 	const int nch = c->cfg.nch, nct = (nch + WB_CTILE - 1) / WB_CTILE;
 	const bool real = c->in_kind == IN_KIND_F32REAL;
 	auto cls = [real](int k) { return real ? ((k & 3) == 0 ? 0 : (k & 3) == 2 ? 1 : 2) : (((k / 2) % 4) + 4) % 4; };
@@ -618,6 +635,23 @@ static int upload_wb_plan(acb_ctx *c, int stream, bool ok, const std::vector<int
 	return ACB_OK;
 }
 
+/* The planners' common tail: the exact tables, `build(ch, wf)` writing channel ch's taps (the low-pass form at taps > K),
+ * then the plan the context's form reads.  `plan(kbin, tw1)` is the input kind's acb_fast_plan* (tw1 NULL: the bins
+ * only), 1 when every channel sits on the raster: otherwise the stream stays on EXACT.  `etab`: upload_wb_plan's. */
+template <class Build, class Plan>
+static int plan_stream(acb_ctx *c, int stream, const Build &build, const Plan &plan, int etab)
+{
+	const int nch = c->cfg.nch, T = c->taps;
+	std::vector<float> wf((size_t)nch * T * 2);
+	for (int ch = 0; ch < nch; ch++) build(ch, &wf[(size_t)ch * T * 2]);
+	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
+	if (c->form == CHAN_EXACT || c->form == CHAN_GENERIC) return ACB_OK;
+	std::vector<int> kbin(nch);
+	if (c->form == CHAN_WB || c->form == CHAN_WB_REAL) return plan(kbin.data(), nullptr) == 1 ? upload_wb_plan(c, stream, kbin, etab) : ACB_OK;
+	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
+	return plan(kbin.data(), tw1.data()) == 1 ? upload_fast_plan(c, stream, kbin, tw1) : ACB_OK;
+}
+
 extern "C" int acb_set_plan(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
@@ -634,22 +668,11 @@ extern "C" int acb_set_plan_at(acb_ctx_t *c, int stream, const unsigned *freqs_h
 	if (c->real_input) return fail(ACB_ERR_ARG, "not a u8-IQ context: use acb_set_plan_air / acb_set_plan_cs16");
 	if (c->taps < c->cfg.K) return fail(ACB_ERR_ARG, "taps < K: the planners build K-tap or low-pass tables only; supply yours with acb_set_wf");
 	if (fc == 0) return fail(ACB_ERR_PLAN, "centre frequency 0");
-	const int T = c->taps;                      /* K, or the low-pass length of an overlapping-window context */
-	std::vector<float> wf((size_t)nch * T * 2);
-	for (int ch = 0; ch < nch; ch++) {
-		if (c->hpad) acb_build_wf_lp(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, T, &wf[(size_t)ch * T * 2]);
-		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
-	}
-	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	const int K = c->cfg.K, N2 = K / 4;
-	std::vector<int> kbin(nch);
-	if (c->wb) return upload_wb_plan(c, stream, acb_fast_plan(freqs_hz, nch, K, fc, kbin.data(), nullptr) == 1, kbin, 0);
-	if (!c->fast && !c->fast_ovl) return ACB_OK;
-	/* Fast forms (taps = K, or the overlapping window's polyphase form): per-channel bin numbers and twiddles, when every
-	 * channel sits on the raster */
-	std::vector<float> tw1((size_t)nch * N2 * 2);
-	const bool ok = acb_fast_plan(freqs_hz, nch, K, fc, kbin.data(), tw1.data()) == 1;
-	return upload_fast_plan(c, stream, ok, kbin, tw1);
+	const int K = c->cfg.K, T = c->taps;        /* K, or the low-pass length of an overlapping-window context */
+	return plan_stream(c, stream, [&](int ch, float *wf) {
+		if (c->hpad) acb_build_wf_lp(acb_stored_fr(freqs_hz[ch]), fc, K, T, wf);
+		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, K, wf);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan(freqs_hz, nch, K, fc, kbin, tw1); }, 0);
 }
 
 static EvTriple get_events(acb_ctx *c)
@@ -917,14 +940,13 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		/* K1 may overwrite d_dm[b] only after the demod of NPIPE submits ago has read it */
 		if (c->dm_used[b]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_dm_free[b], 0));
 		CU(cudaEventRecord(t.ev.a, c->s_comp));
-		int r = 0;
-		/* whole 1024-row blocks through the pipeline kernel, the remaining rows (submits of 4-byte
-		 * samples may carry any count) and unaligned K through the generic one */
-		const int fast = c->use_generic ? 0 : nsamp / OUTBLK;
-		bool dft = c->fast || c->fast_ovl || c->wb;  /* every stream planned on the raster? */
-		for (int s = 0; dft && s < c->cfg.nstreams; s++) dft = c->fast_ok[s] != 0;
-		bool all_rows = false;                       /* the fast CS16 kernel takes partial blocks too */
-		bool ovl_fast = false;                       /* the polyphase form ran: it omits the terms before the stream start itself */
+		/* the context's form, or EXACT while a stream is not planned on the raster */
+		bool fast = c->form != CHAN_EXACT && c->form != CHAN_GENERIC;
+		for (int s = 0; fast && s < c->cfg.nstreams; s++) fast = c->fast_ok[s] != 0;
+		const ChanForm form = fast || c->form == CHAN_GENERIC ? c->form : CHAN_EXACT;
+		/* EXACT: whole 1024-row blocks through the block kernel, the remaining rows (submits of 4-byte samples may carry any
+		 * count) through the generic one; GENERIC (unaligned K): every row through the generic one */
+		const int blocks = form == CHAN_GENERIC ? 0 : nsamp / OUTBLK;
 		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
 		 * for the streaming kinds (submit4) */
 		Hist hist{ nullptr, 0, c->hpad, c->pos };
@@ -935,58 +957,48 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			hist.base = d_iq - (size_t)c->hpad * 4;
 			hist.stride = stride;
 		}
-		if (dft && c->wb && c->in_kind == IN_KIND_F32REAL) {
-			/* every row of the submit; at taps > K the history sits right in front of each stream's rows in d_real
-			 * (submit4), zeros after create / reset */
-			r = launch_channelize_wb_real(d_iq, stride, c->hpad, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                              c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-		} else if (dft && c->wb) {
-			/* every row of the submit, CS16 partial blocks included; at taps > K the terms before the stream start are
-			 * omitted in the kernel */
-			r = launch_channelize_wb(c->in_kind, d_iq, stride, hist, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                         c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-			ovl_fast = true;
-		} else if (dft && c->fast_ovl && c->in_kind == IN_KIND_F32REAL) {
+		int r = 0;
+		switch (form) {
+		case CHAN_EXACT:
+		case CHAN_GENERIC:            /* blocks == 0 */
+			if (blocks)
+				r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, blocks,
+				                      (size_t)nsamp, hist, c->s_comp);
+			break;
+		case CHAN_DFT:
+			r = c->in_kind == IN_KIND_CS16IQ
+			        ? launch_channelize_dft_cs16(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp,
+			                                     c->s_comp)
+			        : launch_channelize_dft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, blocks, (size_t)nsamp,
+			                                c->fold8, c->s_comp);
+			break;
+		case CHAN_RDFT:
+			r = launch_channelize_rdft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			break;
+		case CHAN_OVL_FAST:
+			r = launch_channelize_ovl_fast(c->in_kind, d_iq, stride, hist, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			break;
+		case CHAN_OVL_RDFT:
 			/* the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
 			r = launch_channelize_ovl_rdft(d_iq, stride, c->hpad, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
 			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-		} else if (dft && c->fast_ovl) {
-			r = launch_channelize_ovl_fast(c->in_kind, d_iq, stride, hist, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-			ovl_fast = true;
-		} else if (dft && c->in_kind == IN_KIND_F32REAL && !c->use_generic) {
-			r = launch_channelize_rdft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-		} else if (dft && c->in_kind == IN_KIND_CS16IQ && !c->use_generic) {
-			r = launch_channelize_dft_cs16(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-			all_rows = true;
-		} else if (fast && dft) {
-			r = launch_channelize_dft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp, c->fold8, c->s_comp);
-			c->stats.kernel_launches++;
-			c->stats.fast_chan_launches++;
-		} else if (fast) {
-			r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, fast, (size_t)nsamp,
-			                      hist, c->s_comp);
-			c->stats.kernel_launches++;
+			break;
+		case CHAN_WB:
+			/* at taps > K the terms before the stream start are omitted in the kernel */
+			r = launch_channelize_wb(c->in_kind, d_iq, stride, hist, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                         c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			break;
+		case CHAN_WB_REAL:
+			/* at taps > K the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
+			r = launch_channelize_wb_real(d_iq, stride, c->hpad, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
+			                              c->cfg.nstreams, (size_t)nsamp, c->s_comp);
+			break;
 		}
-		if (!r && !all_rows && nsamp > fast * OUTBLK) {
-			const size_t row0 = (size_t)fast * OUTBLK, nrows = (size_t)nsamp - row0;
+		if (fast || blocks) c->stats.kernel_launches++;          /* the fast kernel, or EXACT's block kernel */
+		if (fast) c->stats.fast_chan_launches++;
+		if (!r && !fast && nsamp > blocks * OUTBLK) {
+			const size_t row0 = (size_t)blocks * OUTBLK, nrows = (size_t)nsamp - row0;
 			r = c->hpad ? launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch,
 			                                            c->cfg.nstreams, row0, nrows, (size_t)nsamp, hist, c->s_comp)
 			            : launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
@@ -994,12 +1006,12 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			c->stats.kernel_launches++;
 		}
 		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
-			/* u8 history: the pipeline kernel read zero bytes (-127.37 after conversion) for the samples before the stream
+			/* u8 history: the block kernel read zero bytes (-127.37 after conversion) for the samples before the stream
 			 * start; the rows whose window reaches there — at most ceil(H/K) <= 16 rows of the first submit after
-			 * create / reset — are recomputed with those terms omitted */
+			 * create / reset — are recomputed with those terms omitted (GENERIC and the fast forms omit them themselves) */
 			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
 			const unsigned long long lead = (H + K - 1) / K;
-			if (!r && fast && !ovl_fast && c->pos < lead) {
+			if (!r && form == CHAN_EXACT && c->pos < lead) {
 				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
 				                                  0, (size_t)std::min<unsigned long long>(lead - c->pos, (unsigned long long)nsamp), (size_t)nsamp,
 				                                  hist, c->s_comp);
@@ -1287,21 +1299,12 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 	if (variant != ACB_CS16_SOAPY && variant != ACB_CS16_SDRPLAY) return fail(ACB_ERR_ARG, "unknown CS16 variant");
 	const unsigned fc = fc_hz ? fc_hz : acb_choose_fc(freqs_hz, nch, c->cfg.K);      /* soapy.c:132-136, sdrplay.c:124 */
 	if (fc == 0) return fail(ACB_ERR_PLAN, "Frequencies too far apart");
-	const int T = c->taps;
-	std::vector<float> wf((size_t)nch * T * 2);
-	for (int ch = 0; ch < nch; ch++) {
-		if (c->hpad) acb_cs16_build_wf_lp(variant, freqs_hz[ch], fc, c->cfg.K, T, &wf[(size_t)ch * T * 2]);
-		else acb_cs16_build_wf(variant, freqs_hz[ch], fc, c->cfg.K, &wf[(size_t)ch * T * 2]);
-	}
 	if (fc_out) *fc_out = fc;
-	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	std::vector<int> kbin(nch);
-	if (c->wb)
-		return upload_wb_plan(c, stream, acb_fast_plan_cs16(variant, freqs_hz, nch, c->cfg.K, fc, kbin.data(), nullptr) == 1, kbin, variant);
-	if (!c->fast && !c->fast_ovl) return ACB_OK;
-	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
-	const bool ok = acb_fast_plan_cs16(variant, freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;
-	return upload_fast_plan(c, stream, ok, kbin, tw1);
+	const int K = c->cfg.K, T = c->taps;
+	return plan_stream(c, stream, [&](int ch, float *wf) {
+		if (c->hpad) acb_cs16_build_wf_lp(variant, freqs_hz[ch], fc, K, T, wf);
+		else acb_cs16_build_wf(variant, freqs_hz[ch], fc, K, wf);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan_cs16(variant, freqs_hz, nch, K, fc, kbin, tw1); }, variant);
 }
 
 static int check_plan_air(acb_ctx *c, const unsigned *freqs_hz, int nch)
@@ -1317,18 +1320,10 @@ static int plan_air(acb_ctx *c, int stream, const unsigned *freqs_hz, int nch, u
 {
 	const unsigned rate = (unsigned)c->cfg.K * ACB_INTRATE;
 	const int T = c->taps;
-	std::vector<float> wf((size_t)nch * T * 2);
-	for (int ch = 0; ch < nch; ch++) {
-		if (c->hpad) acb_air_build_wf_lp((int)freqs_hz[ch], (int)fc, rate, T, &wf[(size_t)ch * T * 2]);
-		else acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, &wf[(size_t)ch * T * 2]);
-	}
-	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
-	std::vector<int> kbin(nch);
-	if (c->wb) return upload_wb_plan(c, stream, acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), nullptr) == 1, kbin, 0);
-	if (!c->fast && !c->fast_ovl) return ACB_OK;
-	std::vector<float> tw1((size_t)nch * (c->cfg.K / 4) * 2);
-	const bool ok = acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin.data(), tw1.data()) == 1;
-	return upload_fast_plan(c, stream, ok, kbin, tw1);
+	return plan_stream(c, stream, [&](int ch, float *wf) {
+		if (c->hpad) acb_air_build_wf_lp((int)freqs_hz[ch], (int)fc, rate, T, wf);
+		else acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, wf);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin, tw1); }, 0);
 }
 
 extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
