@@ -124,6 +124,15 @@ ABI = [
     ("acb_set_plan_at", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_uint]),
     ("acb_set_wf", C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int]),
     ("acb_reset", C.c_int, [C.c_void_p]),
+    ("acb_reset_stream", C.c_int, [C.c_void_p, C.c_int]),
+    ("acb_submit_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("acb_submit_device_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("acb_submit_real_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_submit_cs16_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_submit_cs16_planar_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_submit_real_device_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_submit_cs16_device_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_submit_cs16_planar_device_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("acb_submit_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_submit_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_submit_real_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
@@ -151,6 +160,11 @@ ABI = [
     ("acb_multi_submit_cs16_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     ("acb_multi_submit_cs16_planar_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]),
     ("acb_multi_set_emission_groups", C.c_int, [C.c_void_p, C.c_int, C.c_uint64]),
+    ("acb_multi_submit_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("acb_multi_submit_real_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_multi_submit_cs16_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_multi_submit_cs16_planar_host_ragged", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("acb_multi_reset_stream", C.c_int, [C.c_void_p, C.c_int]),
     ("acb_multi_collect", C.c_int, [C.c_void_p]),
     ("acb_multi_sync", C.c_int, [C.c_void_p]),
     ("acb_multi_drain", C.c_int, [C.c_void_p, C.POINTER(Msg), C.c_int]),
@@ -451,8 +465,29 @@ class Context:
     def reset(self) -> None:
         _check(self.lib, self.lib.acb_reset(self.h))
 
-    def submit_host(self, iq, nblk: int, stream_stride: int | None = None) -> None:
-        """iq: uint8 array (nstreams, nblk*block_bytes) or a raw pointer + stride."""
+    def reset_stream(self, stream: int) -> None:
+        """Restart one stream (acb_reset_stream): its chains, carried remainder, history, position and decode counts."""
+        _check(self.lib, self.lib.acb_reset_stream(self.h, stream))
+
+    def _counts(self, counts, dtype):
+        """A per-stream count array for the ragged calls."""
+        c = np.ascontiguousarray(counts, dtype=dtype)
+        assert c.shape == (self.nstreams,), f"counts: one entry per stream ({self.nstreams})"
+        return c
+
+    def _ragged(self, fn, *args, counts) -> np.ndarray:
+        """A ragged streaming call: returns each stream's new envelope rows."""
+        c = self._counts(counts, np.uint64)
+        nout = np.zeros(self.nstreams, dtype=np.uint64)
+        _check(self.lib, fn(self.h, *args, c.ctypes.data, nout.ctypes.data))
+        return nout.astype(np.int64)
+
+    def submit_host(self, iq, nblk: int = 0, stream_stride: int | None = None, counts=None) -> None:
+        """iq: uint8 array (nstreams, nblk*block_bytes) or a raw pointer + stride.  counts: blocks per stream (the
+        ragged call; nblk is then ignored and the array's row pitch is the default stride)."""
+        if counts is not None:
+            c = self._counts(counts, np.int32)
+            nblk = int(c.max())
         if isinstance(iq, np.ndarray):
             assert iq.dtype == np.uint8 and iq.flags.c_contiguous
             ptr = iq.ctypes.data
@@ -460,10 +495,18 @@ class Context:
                 stream_stride = iq.strides[0] if iq.ndim == 2 else nblk * self.block_bytes
         else:
             ptr = iq
-        _check(self.lib, self.lib.acb_submit_host(self.h, ptr, stream_stride, nblk))
+        if counts is not None:
+            _check(self.lib, self.lib.acb_submit_host_ragged(self.h, ptr, stream_stride, c.ctypes.data))
+        else:
+            _check(self.lib, self.lib.acb_submit_host(self.h, ptr, stream_stride, nblk))
 
-    def submit_device(self, dev_ptr: int, nblk: int, stream_stride: int) -> None:
-        _check(self.lib, self.lib.acb_submit_device(self.h, dev_ptr, stream_stride, nblk))
+    def submit_device(self, dev_ptr: int, nblk: int, stream_stride: int, counts=None) -> None:
+        """counts: blocks per stream (the ragged call; nblk is then ignored)."""
+        if counts is not None:
+            c = self._counts(counts, np.int32)
+            _check(self.lib, self.lib.acb_submit_device_ragged(self.h, dev_ptr, stream_stride, c.ctypes.data))
+        else:
+            _check(self.lib, self.lib.acb_submit_device(self.h, dev_ptr, stream_stride, nblk))
 
     def set_plan_air(self, stream: int, freqs_hz) -> int:
         f = np.asarray(freqs_hz, dtype=np.uint32)
@@ -489,11 +532,14 @@ class Context:
         assert stream_stride >= a.shape[1] and (a.shape[0] == 1 or stream_stride == pitch)
         return stream_stride
 
-    def submit_real(self, x: np.ndarray, stream_stride: int | None = None) -> int:
+    def submit_real(self, x: np.ndarray, stream_stride: int | None = None, counts=None):
         """x: float32 (nstreams, nsamples) real samples, rows contiguous; stream s starts stream_stride samples after
-        stream s-1 (default: the array's row pitch).  Returns envelope samples produced per channel."""
+        stream s-1 (default: the array's row pitch).  Returns envelope samples produced per channel.  counts: samples
+        per stream (the ragged call, each <= the row length); returns each stream's new rows."""
         assert x.dtype == np.float32 and x.ndim == 2 and x.shape[0] == self.nstreams
         stride = self._stream_stride(x, 4, stream_stride)
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_real_host_ragged, x.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_real_host(self.h, x.ctypes.data, stride, x.shape[1]))
 
     def set_plan_cs16(self, stream: int, freqs_hz, variant: int, fc_hz: int = 0) -> int:
@@ -502,33 +548,44 @@ class Context:
         _check(self.lib, self.lib.acb_set_plan_cs16(self.h, stream, f.ctypes.data, len(f), variant, fc_hz, C.byref(fc)))
         return fc.value
 
-    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None) -> int:
+    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None, counts=None):
         """iq: int16 (nstreams, nsamples, 2) interleaved I,Q, rows contiguous; stream_stride in complex samples
-        (default: the array's row pitch)."""
+        (default: the array's row pitch).  counts: as submit_real's."""
         assert iq.dtype == np.int16 and iq.ndim == 3 and iq.shape[0] == self.nstreams and iq.shape[2] == 2 and iq.strides[2] == 2
         stride = self._stream_stride(iq, 4, stream_stride)
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_cs16_host_ragged, iq.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_cs16_host(self.h, iq.ctypes.data, stride, iq.shape[1]))
 
-    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None) -> int:
+    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None, counts=None):
         """xi, xq: int16 (nstreams, nsamples) separate I and Q planes (the SDRplay callback's layout), rows contiguous and
-        both planes with the same stream_stride (default: their row pitch)."""
+        both planes with the same stream_stride (default: their row pitch).  counts: as submit_real's."""
         assert xi.dtype == np.int16 and xq.dtype == np.int16 and xi.shape == xq.shape and xi.shape[0] == self.nstreams
         stride = self._stream_stride(xi, 2, stream_stride)
         assert self._stream_stride(xq, 2, stream_stride) == stride
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_cs16_planar_host_ragged, xi.ctypes.data, xq.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, stride, xi.shape[1]))
 
     # the streaming submits with the input in device memory: pointers, `nsamples` and the stream stride in samples, as the
-    # C calls take them; each returns the envelope samples produced per channel
-    def submit_real_device(self, x_dev: int, nsamples: int, stream_stride: int) -> int:
+    # C calls take them; each returns the envelope samples produced per channel, or with `counts` (samples per stream,
+    # nsamples ignored) each stream's new rows
+    def submit_real_device(self, x_dev: int, nsamples: int, stream_stride: int, counts=None):
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_real_device_ragged, x_dev, stream_stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_real_device(self.h, x_dev, stream_stride, nsamples))
 
-    def submit_cs16_device(self, iq_dev: int, nsamples: int, stream_stride: int) -> int:
+    def submit_cs16_device(self, iq_dev: int, nsamples: int, stream_stride: int, counts=None):
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_cs16_device_ragged, iq_dev, stream_stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_cs16_device(self.h, iq_dev, stream_stride, nsamples))
 
-    def submit_cs16_planar_device(self, xi_dev: int, xq_dev: int, nsamples: int, stream_stride: int) -> int:
+    def submit_cs16_planar_device(self, xi_dev: int, xq_dev: int, nsamples: int, stream_stride: int, counts=None):
+        if counts is not None:
+            return self._ragged(self.lib.acb_submit_cs16_planar_device_ragged, xi_dev, xq_dev, stream_stride, counts=counts)
         return _check(self.lib, self.lib.acb_submit_cs16_planar_device(self.h, xi_dev, xq_dev, stream_stride, nsamples))
 
-    def submit_tensor(self, x, xq=None) -> int:
+    def submit_tensor(self, x, xq=None, counts=None):
         """The device submits from torch CUDA tensors: float32 (nstreams, n) for a real-input context, int16
         (nstreams, n, 2) interleaved or two int16 (nstreams, n) planes (x = I, xq = Q) for a CS16 context.  Rows may be
         views into wider rows (their pitch is the stream stride); samples within a row are contiguous."""
@@ -550,11 +607,13 @@ class Context:
         if not ok:
             raise ValueError(f"expected {layout}, {self.nstreams} streams, samples contiguous within a row")
         stride = x.stride(0) // per if x.shape[0] > 1 else n
+        if counts is not None:           # the ragged calls: samples per stream, each <= n
+            assert int(np.max(counts)) <= n
         if xq is not None:
-            return self.submit_cs16_planar_device(x.data_ptr(), xq.data_ptr(), n, stride)
+            return self.submit_cs16_planar_device(x.data_ptr(), xq.data_ptr(), n, stride, counts=counts)
         if x.dtype == torch.float32:
-            return self.submit_real_device(x.data_ptr(), n, stride)
-        return self.submit_cs16_device(x.data_ptr(), n, stride)
+            return self.submit_real_device(x.data_ptr(), n, stride, counts=counts)
+        return self.submit_cs16_device(x.data_ptr(), n, stride, counts=counts)
 
     def set_emission_groups(self, unit: int, period: int = 0) -> None:
         """unit: 0 per submit, 1 every `period` envelope samples, 2 per transfer of `period` input samples."""
@@ -712,10 +771,29 @@ class MultiContext:
         wf = np.ascontiguousarray(wf, dtype=np.float32)
         _check(self.lib, self.lib.acb_multi_set_wf(self.h, stream, wf.ctypes.data, wf.shape[0]))
 
-    def submit_host(self, iq: np.ndarray, nblk: int) -> None:
+    def submit_host(self, iq: np.ndarray, nblk: int = 0, counts=None) -> None:
+        """counts: blocks per stream (the ragged call; nblk is then ignored)."""
         assert iq.dtype == np.uint8 and iq.flags.c_contiguous
+        if counts is not None:
+            c = np.ascontiguousarray(counts, dtype=np.int32)
+            assert c.shape == (self.nstreams,)
+            nblk = int(c.max())
         stride = iq.strides[0] if iq.ndim == 2 else nblk * OUTBLK * self.K * 2
-        _check(self.lib, self.lib.acb_multi_submit_host(self.h, iq.ctypes.data, stride, nblk))
+        if counts is not None:
+            _check(self.lib, self.lib.acb_multi_submit_host_ragged(self.h, iq.ctypes.data, stride, c.ctypes.data))
+        else:
+            _check(self.lib, self.lib.acb_multi_submit_host(self.h, iq.ctypes.data, stride, nblk))
+
+    def reset_stream(self, stream: int) -> None:
+        """acb_multi_reset_stream: collects the submits in flight, then restarts one stream on the parts serving it."""
+        _check(self.lib, self.lib.acb_multi_reset_stream(self.h, stream))
+
+    def _ragged(self, fn, *args, counts) -> np.ndarray:
+        c = np.ascontiguousarray(counts, dtype=np.uint64)
+        assert c.shape == (self.nstreams,), f"counts: one entry per stream ({self.nstreams})"
+        nout = np.zeros(self.nstreams, dtype=np.uint64)
+        _check(self.lib, fn(self.h, *args, c.ctypes.data, nout.ctypes.data))
+        return nout.astype(np.int64)
 
     def set_plan_air(self, stream: int, freqs_hz) -> int:
         """Real input: Fc chosen once over all channels (acb_air_choose_fc), every part planned around it."""
@@ -730,21 +808,27 @@ class MultiContext:
         _check(self.lib, self.lib.acb_multi_set_plan_cs16(self.h, stream, f.ctypes.data, len(f), variant, fc_hz, C.byref(fc)))
         return fc.value
 
-    # the streaming submits take what Context's take, with the same stride rules
-    def submit_real(self, x: np.ndarray, stream_stride: int | None = None) -> int:
+    # the streaming submits take what Context's take, with the same stride rules (counts: the ragged calls, as Context's)
+    def submit_real(self, x: np.ndarray, stream_stride: int | None = None, counts=None):
         assert x.dtype == np.float32 and x.ndim == 2 and x.shape[0] == self.nstreams
         stride = Context._stream_stride(x, 4, stream_stride)
+        if counts is not None:
+            return self._ragged(self.lib.acb_multi_submit_real_host_ragged, x.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_multi_submit_real_host(self.h, x.ctypes.data, stride, x.shape[1]))
 
-    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None) -> int:
+    def submit_cs16(self, iq: np.ndarray, stream_stride: int | None = None, counts=None):
         assert iq.dtype == np.int16 and iq.ndim == 3 and iq.shape[0] == self.nstreams and iq.shape[2] == 2 and iq.strides[2] == 2
         stride = Context._stream_stride(iq, 4, stream_stride)
+        if counts is not None:
+            return self._ragged(self.lib.acb_multi_submit_cs16_host_ragged, iq.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_multi_submit_cs16_host(self.h, iq.ctypes.data, stride, iq.shape[1]))
 
-    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None) -> int:
+    def submit_cs16_planar(self, xi: np.ndarray, xq: np.ndarray, stream_stride: int | None = None, counts=None):
         assert xi.dtype == np.int16 and xq.dtype == np.int16 and xi.shape == xq.shape and xi.shape[0] == self.nstreams
         stride = Context._stream_stride(xi, 2, stream_stride)
         assert Context._stream_stride(xq, 2, stream_stride) == stride
+        if counts is not None:
+            return self._ragged(self.lib.acb_multi_submit_cs16_planar_host_ragged, xi.ctypes.data, xq.ctypes.data, stride, counts=counts)
         return _check(self.lib, self.lib.acb_multi_submit_cs16_planar_host(self.h, xi.ctypes.data, xq.ctypes.data, stride, xi.shape[1]))
 
     def set_emission_groups(self, unit: int, period: int = 0) -> None:

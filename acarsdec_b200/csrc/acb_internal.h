@@ -106,13 +106,16 @@ int launch_channelize_generic(int mode, const void *in, size_t stream_stride, co
 int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
                                   int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
                                   const Hist &h, CUstream_st *stream);
+/* nrows != NULL (device array): the ragged form, stream s demodulates its first nrows[s] <= nsamp rows (lanes 1, 2, 4 or 8
+ * only: anything else returns cudaErrorInvalidValue) */
 int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                 RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, CUstream_st *stream);
+                 RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, CUstream_st *stream, const int *nrows = nullptr);
 /* The counting form (ACB_FLAG_DECODE_STATS): the same demodulator, and chain g adds its frame synchroniser's events to
  * counts[g * EV_COUNT + e] (frame_sm.h; the caller clears them).  Lanes 1, 2, 4 or 8 only (the default forms): anything
  * else returns cudaErrorInvalidValue and launches nothing. */
 int launch_demod_stats(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, unsigned *counts, CUstream_st *stream);
+                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, unsigned *counts, CUstream_st *stream,
+                       const int *nrows = nullptr);
 int demod_pick_lanes(long long nchains, int sm_count);
 bool channelize_dft_supports(int K);
 int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
@@ -139,6 +142,15 @@ int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_st
  * (interleaved on the way), source rows `src_stride` samples apart, to out + s*out_stride (any 4-byte alignment) */
 int launch_append4(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, size_t nsamples, int nstreams,
                    CUstream_st *stream);
+/* Ragged submits (device arrays, one entry per stream): the append lands count[s] samples at out + s*out_stride + off[s];
+ * the tail move copies stream s's hpad + rem[s] samples from row nrows[s] to the front of the other buffer; the history
+ * gather takes each u8 stream's last hb bytes at nblk[s] blocks (a stream with none keeps its history) */
+int launch_append4_ragged(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, const int *off,
+                          const int *count, size_t max_count, int nstreams, CUstream_st *stream);
+int launch_move_tail(const uint32_t *src, uint32_t *dst, size_t stride, int K, int hpad, const int *nrows, const int *rem,
+                     int nstreams, CUstream_st *stream);
+int launch_hist_gather(const uint8_t *in, size_t stride, size_t blk_bytes, const int *nblk, uint8_t *hist, int hb, int nstreams,
+                       CUstream_st *stream);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
 
@@ -148,6 +160,9 @@ int fail(int code, const char *fmt, ...);
 /* Emission-group starts of a streaming submit that covers envelope samples [pos, pos + nout): the first is pos, then
  * one per `period` outputs (ACB_GROUP_OUTPUTS) or per transfer of `period` input samples (ACB_GROUP_INPUT) */
 std::vector<unsigned long long> stream_groups(int unit, unsigned long long period, int K, unsigned long long pos, size_t nout);
+/* The number, counted from the stream's start, of the emission group that holds envelope sample `pos` (u8: its 1024-row
+ * block; the streaming kinds: the group of stream_groups, none for ACB_GROUP_SUBMIT) */
+unsigned long long group_number(bool u8, int unit, unsigned long long period, int K, unsigned long long pos);
 } // namespace acb
 
 #endif

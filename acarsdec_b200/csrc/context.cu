@@ -90,12 +90,27 @@ constexpr int NPIPE = 3;
  * submit runs EXACT otherwise. */
 enum ChanForm { CHAN_EXACT, CHAN_GENERIC, CHAN_DFT, CHAN_RDFT, CHAN_OVL_FAST, CHAN_OVL_RDFT, CHAN_WB, CHAN_WB_REAL };
 
+/* Emission-order groups of one submit (input blocks / chunks).  Even submits (every stream at the same position):
+ * `starts` holds the groups every stream shares and `off` is empty.  Otherwise stream s's groups are
+ * starts[off[s] .. off[s+1]), and base[s] is the number, counted from the stream's own start, of its first one: frames
+ * leave in (that number, stream, channel, time) order. */
+struct Groups {
+	std::vector<unsigned long long> starts;
+	std::vector<unsigned> off;
+	std::vector<unsigned long long> base;
+};
+
 /* one submit in flight: which frame ring it appends to and how its frames are grouped */
 struct Ticket {
 	EvTriple ev;                                   /* a..b = channelizer, b..c = demod; c = done */
 	int ring;
-	std::vector<unsigned long long> group_starts;  /* emission-order groups (input blocks / chunks) */
+	Groups groups;
+	unsigned long long seq;                        /* the submit's number (acb_ctx::nsubmit when it was made) */
 };
+
+/* Ragged submits' per-stream counts on the device: slots of 4 * nstreams ints (rows | a | b | c, see stage_begin), reused
+ * round robin once the work that read them is done */
+constexpr int NRAG = NPIPE + 1;
 
 struct acb_ctx {
 	acb_config_t cfg;
@@ -133,7 +148,7 @@ struct acb_ctx {
 	RingCtl *h_ctl[NPIPE];       /* pinned */
 	int last_nsamp;
 	unsigned long long nsubmit;
-	unsigned long long pos;      /* envelope samples submitted so far (all chains move together) */
+	std::vector<unsigned long long> pos;   /* per stream: envelope samples submitted since create / reset */
 	std::deque<Ticket> inflight; /* oldest first; at most NPIPE */
 	/* output queue: one batch per harvested submit, already in emission order; drained by bulk copies (at a
 	 * Tsample/s a step carries tens of thousands of messages: per-message queue operations were the host's
@@ -142,7 +157,7 @@ struct acb_ctx {
 	std::deque<Batch> outq;
 	size_t outq_count;
 	/* consumer thread: everything from `outq` to `jobs_done`, plus stats.raw_frames / fec_dropped, is guarded by mtx */
-	struct Job { std::vector<unsigned long long> group_starts; int ring; unsigned count; };
+	struct Job { Groups groups; int ring; unsigned count; unsigned long long seq; };
 	std::thread consumer;
 	std::mutex mtx;
 	std::condition_variable cv_job, cv_done;
@@ -163,7 +178,7 @@ struct acb_ctx {
 	bool real_input;             /* in_kind != u8: 4-byte input elements, arbitrary submit lengths, carried remainder */
 	float *d_real[2];            /* per stream: [hpad history + carry + new samples], alternating per submit */
 	size_t real_cap;             /* floats per stream in d_real */
-	size_t carry;                /* samples of every stream not yet consumed (< K) */
+	std::vector<size_t> carry;   /* per stream: samples not yet consumed (< K) */
 	int real_buf;
 	cudaEvent_t ev_real_copied, ev_real_free[2];   /* H2D of a streaming submit landed | d_real[b] may be overwritten */
 	bool real_used[2];
@@ -182,6 +197,11 @@ struct acb_ctx {
 	unsigned *d_evcnt[NPIPE];
 	unsigned *h_evcnt[NPIPE];    /* pinned */
 	std::vector<acb_decode_stats_t> dstats;      /* guarded by dstats_mtx */
+	std::vector<unsigned long long> dstats_from; /* per stream: the first submit its counts cover (acb_reset_stream); dstats_mtx */
+	int *d_rag[NRAG], *h_rag[NRAG];               /* ragged submits' counts (h_rag pinned) */
+	cudaEvent_t ev_rag_used[NRAG][3];             /* behind the last reads of slot i on the copy, channelizer and demod streams */
+	bool rag_used[NRAG];
+	unsigned long long rag_seq;
 };
 
 static void consumer_main(acb_ctx *c);
@@ -263,8 +283,8 @@ static int reset_states(acb_ctx *c)
 		for (int i = 0; i < 2; i++)
 			CU(cudaMemset2DAsync(c->d_real[i], c->real_cap * sizeof(float), 0, (size_t)c->hpad * sizeof(float), c->cfg.nstreams, c->s_copy));
 	CU(cudaStreamSynchronize(c->s_copy));
-	c->pos = 0;
-	c->carry = 0;
+	c->pos.assign(c->cfg.nstreams, 0);
+	c->carry.assign(c->cfg.nstreams, 0);
 	{
 		std::lock_guard<std::mutex> lk(c->mtx);
 		c->outq.clear();
@@ -348,7 +368,6 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->s_order = nullptr;
 	c->ev_order = nullptr;
 	c->order_pending = false;
-	c->carry = 0;
 	c->real_buf = 0;
 	c->group_unit = ACB_GROUP_SUBMIT;
 	c->group_period = 0;
@@ -363,6 +382,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->h_ring[0] = c->h_ring[1] = nullptr;
 	c->overflowed = false;
 	memset(&c->stats, 0, sizeof(c->stats));
+	for (int i = 0; i < NRAG; i++) c->d_rag[i] = nullptr, c->h_rag[i] = nullptr;
 	c->decode_stats = (cfg->flags & ACB_FLAG_DECODE_STATS) != 0;
 	for (int i = 0; i < NPIPE; i++) c->d_evcnt[i] = nullptr, c->h_evcnt[i] = nullptr;
 	*out = c;
@@ -488,10 +508,18 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	for (int i = 0; i < NPIPE; i++) CU(cudaHostAlloc(&c->h_ring[i], cap * sizeof(RawFrame), cudaHostAllocDefault));
 	if (c->decode_stats) {
 		c->dstats.assign(nchain, acb_decode_stats_t{});
+		c->dstats_from.assign(cfg->nstreams, 0);
 		for (int i = 0; i < NPIPE; i++) {
 			CU(cudaMalloc(&c->d_evcnt[i], nchain * EV_COUNT * sizeof(unsigned)));
 			CU(cudaHostAlloc(&c->h_evcnt[i], nchain * EV_COUNT * sizeof(unsigned), cudaHostAllocDefault));
 		}
+	}
+	c->rag_seq = 0;
+	for (int i = 0; i < NRAG; i++) {
+		CU(cudaMalloc(&c->d_rag[i], 4 * (size_t)cfg->nstreams * sizeof(int)));
+		CU(cudaHostAlloc(&c->h_rag[i], 4 * (size_t)cfg->nstreams * sizeof(int), cudaHostAllocDefault));
+		for (auto &e : c->ev_rag_used[i]) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+		c->rag_used[i] = false;
 	}
 	c->consumer = std::thread(consumer_main, c);
 
@@ -543,6 +571,11 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 			cudaFree(c->d_ring[i]); cudaFree(c->d_ctl[i]); cudaFreeHost(c->h_ctl[i]); cudaFreeHost(c->h_ring[i]);
 			cudaFree(c->d_evcnt[i]); cudaFreeHost(c->h_evcnt[i]);
 		}
+		for (int i = 0; i < NRAG; i++) {
+			if (!c->d_rag[i]) continue;
+			cudaFree(c->d_rag[i]); cudaFreeHost(c->h_rag[i]);
+			for (auto &e : c->ev_rag_used[i]) cudaEventDestroy(e);
+		}
 		cudaEventDestroy(c->mark[0]); cudaEventDestroy(c->mark[1]); cudaEventDestroy(c->ev_join);
 		cudaStreamDestroy(c->s_copy); cudaStreamDestroy(c->s_comp); cudaStreamDestroy(c->s_dem); cudaStreamDestroy(c->s_fec); cudaStreamDestroy(c->s_d2h);
 	}
@@ -561,6 +594,35 @@ extern "C" int acb_reset(acb_ctx_t *c)
 	for (int i = 0; i < NPIPE; i++) c->ring_read_pending[i] = false;
 	for (int i = 0; i < NPIPE; i++) c->k1_pending[i] = false;
 	return reset_states(c);
+}
+
+extern "C" int acb_reset_stream(acb_ctx_t *c, int stream)
+{
+	if (!c) return fail(ACB_ERR_ARG, "null context");
+	if (stream < 0 || stream >= c->cfg.nstreams) return fail(ACB_ERR_ARG, "stream %d out of range", stream);
+	if (int r = ctx_use(c)) return r;
+	/* initMsk + initAcars (reset_states), behind the demods already queued and ahead of the next */
+	ChainState *st = c->d_state + (size_t)stream * c->cfg.nch;
+	CU(cudaMemsetAsync(st, 0, (size_t)c->cfg.nch * sizeof(ChainState), c->s_dem));
+	static_assert(offsetof(ChainState, nbits) % 4 == 0, "nbits: an int whose low byte is set alone (little endian)");
+	CU(cudaMemset2DAsync(&st->nbits, sizeof(ChainState), 8, 1, c->cfg.nch, c->s_dem));
+	/* the history, behind the channelizer and tail move that wrote it: the next submit's rows of this stream start at row 0 */
+	if (c->d_hist) CU(cudaMemsetAsync(c->d_hist + (size_t)stream * c->hpad * 2, 0, (size_t)c->hpad * 2, c->s_comp));
+	if (c->hpad && c->real_input)
+		CU(cudaMemsetAsync(c->d_real[c->real_buf] + (size_t)stream * c->real_cap, 0, (size_t)c->hpad * sizeof(float), c->s_comp));
+	if (c->real_input) {
+		/* the next append lands where the tail move put the discarded remainder: it must come after it */
+		CU(cudaEventRecord(c->ev_join, c->s_comp));
+		CU(cudaStreamWaitEvent(c->s_copy, c->ev_join, 0));
+	}
+	c->pos[stream] = 0;
+	if (c->real_input) c->carry[stream] = 0;
+	if (c->decode_stats) {
+		std::lock_guard<std::mutex> lk(c->dstats_mtx);
+		memset(&c->dstats[(size_t)stream * c->cfg.nch], 0, (size_t)c->cfg.nch * sizeof(acb_decode_stats_t));
+		c->dstats_from[stream] = c->nsubmit;
+	}
+	return ACB_OK;
 }
 
 extern "C" int acb_set_wf(acb_ctx_t *c, int stream, const float *wf, int nch)
@@ -704,7 +766,10 @@ static void add_decode_stats(acb_ctx *c, const acb_ctx::Job &job, const RawFrame
 	std::lock_guard<std::mutex> lk(c->dstats_mtx);
 	const size_t nchain = c->dstats.size();
 	const unsigned *ev = c->h_evcnt[job.ring];
+	/* a stream reset after this submit was made (acb_reset_stream) counts from its next submit on */
+	auto counted = [c, &job](size_t stream) { return job.seq >= c->dstats_from[stream]; };
 	for (size_t g = 0; g < nchain; g++) {
+		if (!counted(g / c->cfg.nch)) continue;
 		const unsigned *e = ev + g * EV_COUNT;
 		acb_decode_stats_t &d = c->dstats[g];
 		d.preamble += e[EV_PREAMBLE];
@@ -718,6 +783,7 @@ static void add_decode_stats(acb_ctx *c, const acb_ctx::Job &job, const RawFrame
 	}
 	for (unsigned i = 0; i < job.count; i++) {
 		const RawFrame &f = ring[i];
+		if (!counted((size_t)f.stream)) continue;
 		const unsigned why = f.pad1[0];
 		acb_decode_stats_t &d = c->dstats[(size_t)f.stream * c->cfg.nch + f.chn];
 		d.fec_parity_excess += (why & FEC_WHY_PARITY_EXCESS) != 0;
@@ -733,7 +799,7 @@ static void add_decode_stats(acb_ctx *c, const acb_ctx::Job &job, const RawFrame
 static void consume(acb_ctx *c, const acb_ctx::Job &job)
 {
 	const unsigned count = job.count;
-	const auto &gs = job.group_starts;
+	const auto &gs = job.groups.starts;
 	const RawFrame *ring = c->h_ring[job.ring];
 	/* emission order = (group, stream, channel, time).  A chain's frames reach the ring in time order (one thread
 	 * appends them as it decodes), so a STABLE bucket pass over (group, chain) is the whole sort: O(frames + buckets)
@@ -747,7 +813,52 @@ static void consume(acb_ctx *c, const acb_ctx::Job &job)
 	/* test hooks (tests/test_gpu_parity.py): ACB_CONSUMER_SORT=1 forces the comparison sort, ACB_CONSUMER_HELPERS_MIN=n the
 	 * helper threads from n frames on */
 	const bool force_sort = getenv("ACB_CONSUMER_SORT") && atoi(getenv("ACB_CONSUMER_SORT")) != 0;
-	if (!force_sort && nbucket <= ((size_t)1 << 24)) {
+	if (!job.groups.off.empty()) {
+		/* streams at different positions: each (stream, group) pair of the submit gets its rank in (group number counted
+		 * from the stream's start, stream) order; then the bucket pass (or the comparison sort) as below, over
+		 * (rank, channel) */
+		const auto &off = job.groups.off;
+		const auto &base = job.groups.base;
+		const unsigned npair = off.back();
+		std::vector<unsigned> pair_stream(npair), by_key(npair), rank(npair);
+		for (int st = 0; st < c->cfg.nstreams; st++)
+			for (unsigned p = off[st]; p < off[st + 1]; p++) pair_stream[p] = (unsigned)st;
+		auto gnum = [&](unsigned p) { return base[pair_stream[p]] + (p - off[pair_stream[p]]); };
+		for (unsigned p = 0; p < npair; p++) by_key[p] = p;
+		std::sort(by_key.begin(), by_key.end(), [&](unsigned a, unsigned b) {
+			const unsigned long long ga = gnum(a), gb = gnum(b);
+			return ga != gb ? ga < gb : pair_stream[a] < pair_stream[b];
+		});
+		for (unsigned k = 0; k < npair; k++) rank[by_key[k]] = k;
+		/* the pair a frame belongs to: its stream's last group starting at or before it */
+		auto pair_of = [&](const RawFrame &f) {
+			const auto b = gs.begin() + off[f.stream], e = gs.begin() + off[f.stream + 1];
+			const auto it = std::upper_bound(b, e, f.pos);
+			return off[f.stream] + (unsigned)(it == b ? 0 : it - b - 1);
+		};
+		const size_t nb = (size_t)npair * c->cfg.nch;
+		if (!force_sort && nb <= ((size_t)1 << 24)) {
+			std::vector<unsigned> start(nb + 1, 0u), bucket(count);
+			for (unsigned i = 0; i < count; i++) {
+				const RawFrame &f = ring[i];
+				keep[i] = f.pad0 == 1;
+				const size_t bk = (size_t)rank[pair_of(f)] * c->cfg.nch + f.chn;
+				bucket[i] = (unsigned)bk;
+				start[bk + 1]++;
+			}
+			for (size_t k = 0; k < nb; k++) start[k + 1] += start[k];
+			for (unsigned i = 0; i < count; i++) order[start[bucket[i]]++] = i;
+		} else {
+			std::vector<unsigned> rk(count);
+			for (unsigned i = 0; i < count; i++) { order[i] = i; keep[i] = ring[i].pad0 == 1; rk[i] = rank[pair_of(ring[i])]; }
+			std::stable_sort(order.begin(), order.end(), [ring, &rk](unsigned ia, unsigned ib) {
+				const RawFrame &x = ring[ia], &y = ring[ib];
+				if (rk[ia] != rk[ib]) return rk[ia] < rk[ib];
+				if (x.chn != y.chn) return x.chn < y.chn;
+				return x.pos < y.pos;
+			});
+		}
+	} else if (!force_sort && nbucket <= ((size_t)1 << 24)) {
 		std::vector<unsigned> start(nbucket + 1, 0u), bucket(count);
 		for (unsigned i = 0; i < count; i++) {          /* the one pass in ring order: sequential reads */
 			const RawFrame &f = ring[i];
@@ -893,7 +1004,7 @@ static int harvest_begin(acb_ctx *c)
 	c->ring_read_pending[t.ring] = true;
 	{
 		std::lock_guard<std::mutex> lk(c->mtx);
-		c->jobs.push_back(acb_ctx::Job{ std::move(t.group_starts), t.ring, count });
+		c->jobs.push_back(acb_ctx::Job{ std::move(t.groups), t.ring, count, t.seq });
 		c->ring_job[t.ring] = ++c->jobs_queued;
 	}
 	c->cv_job.notify_one();
@@ -909,9 +1020,11 @@ static int collect_oldest(acb_ctx *c)
 	return ACB_OK;
 }
 
-/* queue K1+K2 (or K2 only) on the compute stream for `nblk` blocks / `nsamp` envelope samples */
+/* queue K1+K2 (or K2 only) on the compute stream for `nblk` blocks / `nsamp` envelope samples.  Ragged submits (`rag`, a
+ * slot of stage_counts, and `h_rows` its host copy): stream s has h_rows[s] <= nsamp rows of its own; K1 computes nsamp
+ * rows of every stream, K2 reads each stream's own. */
 static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk, int nsamp, const float *dm_host,
-                       std::vector<unsigned long long> &&groups)
+                       Groups &&groups, const int *rag = nullptr, const int *h_rows = nullptr)
 {
 	/* the ring this submit appends to was last used NPIPE submits ago: its frames must be on their
 	 * way back before the new demod may clear it — but the host-side work on those frames waits
@@ -931,7 +1044,8 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 	}
 	Ticket t;
 	t.ring = (int)(c->nsubmit % NPIPE);
-	t.group_starts = std::move(groups);
+	t.groups = std::move(groups);
+	t.seq = c->nsubmit;
 	t.ev = get_events(c);
 	t.ev.chan = d_iq != nullptr;
 	const int b = t.ring;                          /* envelope buffer and frame ring of this submit */
@@ -949,7 +1063,12 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		const int blocks = form == CHAN_GENERIC ? 0 : nsamp / OUTBLK;
 		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
 		 * for the streaming kinds (submit4) */
-		Hist hist{ nullptr, 0, c->hpad, c->pos };
+		/* streams at different positions (acb_reset_stream): the launch takes the furthest one, and the streams near their
+		 * start whose window reaches before it are redone below, one by one, at their own position */
+		const unsigned long long pos_max = *std::max_element(c->pos.begin(), c->pos.end());
+		const bool even_pos = std::all_of(c->pos.begin(), c->pos.end(), [&](unsigned long long p) { return p == pos_max; });
+		auto rows_of = [&](int s) { return h_rows ? (size_t)h_rows[s] : (size_t)nsamp; };
+		Hist hist{ nullptr, 0, c->hpad, pos_max };
 		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
 			hist.base = c->d_hist;
 			hist.stride = (size_t)c->hpad * 2;
@@ -996,6 +1115,25 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			break;
 		}
 		if (fast || blocks) c->stats.kernel_launches++;          /* the fast kernel, or EXACT's block kernel */
+		if (!r && !even_pos && c->hpad && (form == CHAN_OVL_FAST || form == CHAN_WB)) {
+			/* these forms omit the terms before the stream start themselves, from hist.pos0: a stream whose window still
+			 * reaches there (within (hpad + K - 1) / K rows of its start) is redone alone at its own position */
+			const unsigned long long reach = ((unsigned long long)c->hpad + c->cfg.K - 1) / c->cfg.K;
+			const size_t wf_per = (size_t)c->ngrp * CH_GROUP * (c->cfg.K / 4) * 2;
+			const size_t nct = (size_t)(c->cfg.nch + WB_CTILE - 1) / WB_CTILE;
+			for (int s = 0; !r && s < c->cfg.nstreams; s++) {
+				if (c->pos[s] >= reach || rows_of(s) == 0) continue;
+				Hist h1{ (const uint8_t *)hist.base + (size_t)s * hist.stride, hist.stride, c->hpad, c->pos[s] };
+				const uint8_t *in1 = d_iq + (size_t)s * stride;
+				float *dm1 = dmbuf + (size_t)s * nsamp * c->cfg.nch;
+				r = form == CHAN_OVL_FAST
+				        ? launch_channelize_ovl_fast(c->in_kind, in1, stride, h1, c->d_p, c->d_tw + s * wf_per, c->d_twmeta + (size_t)s * c->ngrp,
+				                                     dm1, c->cfg.K, c->cfg.nch, 1, (size_t)nsamp, c->s_comp)
+				        : launch_channelize_wb(c->in_kind, in1, stride, h1, c->d_p, c->d_wbE, c->d_wbmeta + s * nct * WB_META, dm1, c->cfg.K,
+				                               c->cfg.nch, 1, (size_t)nsamp, c->s_comp);
+				c->stats.kernel_launches++;
+			}
+		}
 		if (fast) c->stats.fast_chan_launches++;
 		if (!r && !fast && nsamp > blocks * OUTBLK) {
 			const size_t row0 = (size_t)blocks * OUTBLK, nrows = (size_t)nsamp - row0;
@@ -1011,16 +1149,31 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 			 * create / reset — are recomputed with those terms omitted (GENERIC and the fast forms omit them themselves) */
 			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
 			const unsigned long long lead = (H + K - 1) / K;
-			if (!r && form == CHAN_EXACT && c->pos < lead) {
+			if (!r && form == CHAN_EXACT && even_pos && pos_max < lead) {
 				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
-				                                  0, (size_t)std::min<unsigned long long>(lead - c->pos, (unsigned long long)nsamp), (size_t)nsamp,
+				                                  0, (size_t)std::min<unsigned long long>(lead - pos_max, (unsigned long long)nsamp), (size_t)nsamp,
 				                                  hist, c->s_comp);
+				c->stats.kernel_launches++;
+			}
+			/* streams at different positions: EXACT's block kernel and GENERIC's launch (at pos_max) took the zero history
+			 * bytes as terms; redo the rows of each stream that reach before its start, stream by stream, at its own position */
+			const bool redo = form == CHAN_EXACT || form == CHAN_GENERIC;
+			for (int s = 0; !r && redo && !even_pos && s < c->cfg.nstreams; s++) {
+				if (c->pos[s] >= lead || rows_of(s) == 0) continue;
+				const Hist h1{ c->d_hist + (size_t)s * hist.stride, hist.stride, c->hpad, c->pos[s] };
+				r = launch_channelize_generic_ovl(c->in_kind, d_iq + (size_t)s * stride, stride,
+				                                  c->d_wf + (size_t)s * c->ngrp * c->taps_pad * CH_GROUP * 2, dmbuf + (size_t)s * nsamp * c->cfg.nch,
+				                                  c->cfg.K, c->taps_pad, c->cfg.nch, 1, 0,
+				                                  std::min<size_t>(lead - c->pos[s], rows_of(s)), (size_t)nsamp, h1, c->s_comp);
 				c->stats.kernel_launches++;
 			}
 			/* the input's last hpad samples are the next submit's history; the copy follows K1 on the same stream, so
 			 * K1 of the next submit sees it and the input-lifetime event below covers it */
 			const size_t hb = (size_t)c->hpad * 2, len = (size_t)nblk * c->blk_bytes;
-			if (!r) {
+			if (!r && rag) {
+				r = launch_hist_gather(d_iq, stride, c->blk_bytes, rag + c->cfg.nstreams, c->d_hist, (int)hb, c->cfg.nstreams, c->s_comp);
+				c->stats.kernel_launches++;
+			} else if (!r) {
 				r = c->cfg.nstreams == 1 ? (int)cudaMemcpyAsync(c->d_hist, d_iq + len - hb, hb, cudaMemcpyDeviceToDevice, c->s_comp)
 				                         : (int)cudaMemcpy2DAsync(c->d_hist, hb, d_iq + len - hb, stride, hb, c->cfg.nstreams,
 				                                                  cudaMemcpyDeviceToDevice, c->s_comp);
@@ -1045,9 +1198,9 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 	if (c->decode_stats) CU(cudaMemsetAsync(c->d_evcnt[b], 0, c->dstats.size() * EV_COUNT * sizeof(unsigned), c->s_dem));
 	CU(cudaEventRecord(t.ev.b2, c->s_dem));
 	int r = c->decode_stats ? launch_demod_stats(c->d_state, dmbuf, nsamp, c->cfg.nch, c->cfg.nstreams, c->d_ring[b], c->d_ctl[b],
-	                                             c->ring_cap, c->demod_lanes, c->d_evcnt[b], c->s_dem)
+	                                             c->ring_cap, c->demod_lanes, c->d_evcnt[b], c->s_dem, rag)
 	                        : launch_demod(c->d_state, dmbuf, nsamp, c->cfg.nch, c->cfg.nstreams, c->d_ring[b], c->d_ctl[b], c->ring_cap,
-	                                       c->demod_lanes, c->s_dem);
+	                                       c->demod_lanes, c->s_dem, rag);
 	if (r) return fail(ACB_ERR_CUDA, "demod launch: %s", cudaGetErrorString((cudaError_t)r));
 	c->stats.kernel_launches++;
 	c->stats.demod_launches++;
@@ -1081,47 +1234,184 @@ static int check_blocks(acb_ctx *c, const void *p, size_t stride, int nblk)
 	return ACB_OK;
 }
 
-static std::vector<unsigned long long> block_groups(const acb_ctx *c, int nblk)
+/* the ragged calls' counts: each 0..max_blocks, not all 0; `maxb` = the largest, which the stride must hold */
+static int check_blocks_ragged(acb_ctx *c, const void *p, size_t stride, const int *nblk, int &maxb)
 {
-	std::vector<unsigned long long> g(nblk);
-	for (int b = 0; b < nblk; b++) g[b] = c->pos + (unsigned long long)b * OUTBLK;
+	if (!c || !p || !nblk) return fail(ACB_ERR_ARG, "null argument");
+	if (c->real_input) return fail(ACB_ERR_ARG, "not a u8-IQ context: use acb_submit_real_host_ragged / acb_submit_cs16_host_ragged");
+	maxb = 0;
+	for (int s = 0; s < c->cfg.nstreams; s++) {
+		if (nblk[s] < 0 || nblk[s] > c->cfg.max_blocks) return fail(ACB_ERR_ARG, "nblk[%d]=%d outside 0..%d", s, nblk[s], c->cfg.max_blocks);
+		maxb = std::max(maxb, nblk[s]);
+	}
+	if (maxb == 0) return fail(ACB_ERR_ARG, "every stream's nblk is 0");
+	if (c->cfg.nstreams > 1 && stride < (size_t)maxb * c->blk_bytes) return fail(ACB_ERR_ARG, "stream_stride smaller than the largest input");
+	if (stride % 16) return fail(ACB_ERR_ARG, "stream_stride must be a multiple of 16 bytes");
+	return ACB_OK;
+}
+
+/* The number, counted from the stream's start, of the emission group that holds envelope sample `pos`: its 1024-row block
+ * (u8), or the groups of stream_groups — one per `period` outputs (ACB_GROUP_OUTPUTS), or the first output completed in
+ * each transfer of `period` input samples (ACB_GROUP_INPUT: the transfers' first outputs floor(t*T/K), t >= 1, in (0, pos]);
+ * ACB_GROUP_SUBMIT has one group per submit and numbers none. */
+unsigned long long acb::group_number(bool u8, int unit, unsigned long long period, int Kc, unsigned long long pos)
+{
+	if (u8) return pos / OUTBLK;
+	const unsigned long long T = period, K = (unsigned long long)Kc;
+	if (unit == ACB_GROUP_OUTPUTS) return pos / T;
+	if (unit == ACB_GROUP_INPUT) return T >= K ? ((pos + 1) * K - 1) / T : pos;
+	return 0;
+}
+
+/* The emission groups of a submit in which stream s brings rows[s] envelope rows (u8: whole blocks of 1024) */
+static Groups submit_groups(const acb_ctx *c, const std::vector<size_t> &rows)
+{
+	auto of = [c](unsigned long long pos, size_t n) {
+		if (c->real_input) return stream_groups(c->group_unit, c->group_period, c->cfg.K, pos, n);
+		std::vector<unsigned long long> g(n / OUTBLK);
+		for (size_t b = 0; b < g.size(); b++) g[b] = pos + (unsigned long long)b * OUTBLK;
+		return g;
+	};
+	Groups g;
+	const int n = c->cfg.nstreams;
+	if (std::all_of(c->pos.begin(), c->pos.end(), [c](unsigned long long p) { return p == c->pos[0]; })) {
+		g.starts = of(c->pos[0], *std::max_element(rows.begin(), rows.end()));
+		return g;
+	}
+	g.off.assign(n + 1, 0u);
+	g.base.assign(n, 0ull);
+	for (int s = 0; s < n; s++) {
+		if (rows[s]) {
+			const auto v = of(c->pos[s], rows[s]);
+			g.starts.insert(g.starts.end(), v.begin(), v.end());
+			g.base[s] = group_number(!c->real_input, c->group_unit, c->group_period, c->cfg.K, c->pos[s]);
+		}
+		g.off[s + 1] = (unsigned)g.starts.size();
+	}
 	return g;
+}
+
+/* Ragged submits' counts travel in a slot of 4 * nstreams ints: [rows | a | b | c], where u8 puts its block counts in a
+ * and the streaming kinds each stream's carry, new samples and remainder in a, b, c.  stage_begin hands out the next
+ * slot once the work that read it last is done; stage_upload copies it on the copy stream and orders the channelizer
+ * stream behind it; stage_end marks the streams that read it. */
+static int stage_begin(acb_ctx *c, int &slot)
+{
+	slot = (int)(c->rag_seq++ % NRAG);
+	if (c->rag_used[slot])
+		for (auto &e : c->ev_rag_used[slot]) CU(cudaEventSynchronize(e));
+	c->rag_used[slot] = false;
+	return ACB_OK;
+}
+
+static int stage_upload(acb_ctx *c, int slot)
+{
+	CU(cudaMemcpyAsync(c->d_rag[slot], c->h_rag[slot], 4 * (size_t)c->cfg.nstreams * sizeof(int), cudaMemcpyHostToDevice, c->s_copy));
+	CU(cudaEventRecord(c->ev_rag_used[slot][0], c->s_copy));
+	CU(cudaStreamWaitEvent(c->s_comp, c->ev_rag_used[slot][0], 0));
+	return ACB_OK;
+}
+
+static int stage_end(acb_ctx *c, int slot)
+{
+	CU(cudaEventRecord(c->ev_rag_used[slot][0], c->s_copy));
+	CU(cudaEventRecord(c->ev_rag_used[slot][1], c->s_comp));
+	CU(cudaEventRecord(c->ev_rag_used[slot][2], c->s_dem));
+	c->rag_used[slot] = true;
+	return ACB_OK;
+}
+
+/* Host rows of `elem`-byte samples into a device buffer of row pitch `dpitch`: stream s brings cnt[s].  Even counts are
+ * one 2D copy.  Otherwise every stream but the last is copied at the largest count (its row in the caller's buffer is at
+ * least that long: the stride holds it) and the last at its own, so nothing past the caller's input is read. */
+static int copy_rows(acb_ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, const std::vector<size_t> &cnt, size_t elem,
+                     bool even)
+{
+	const int n = c->cfg.nstreams;
+	if (even) {
+		CU(cudaMemcpy2DAsync(dst, dpitch, src, spitch, cnt[0] * elem, n, cudaMemcpyHostToDevice, c->s_copy));
+		return ACB_OK;
+	}
+	const size_t wmax = *std::max_element(cnt.begin(), cnt.end()) * elem;
+	CU(cudaMemcpy2DAsync(dst, dpitch, src, spitch, wmax, n - 1, cudaMemcpyHostToDevice, c->s_copy));
+	if (cnt[n - 1])
+		CU(cudaMemcpyAsync((char *)dst + (size_t)(n - 1) * dpitch, (const char *)src + (size_t)(n - 1) * spitch, cnt[n - 1] * elem,
+		                   cudaMemcpyHostToDevice, c->s_copy));
+	return ACB_OK;
+}
+
+/* u8 IQ submits: `nblk` blocks for every stream, or (nblk_s != NULL, the ragged calls) nblk_s[s] for stream s, nblk the
+ * largest.  The channelizer runs nblk blocks of every stream; each stream's demodulator takes its own. */
+static int submit_blocks(acb_ctx *c, const uint8_t *iq, size_t stride, int nblk, const int *nblk_s, bool dev)
+{
+	if (int r = ctx_use(c)) return r;
+	if (dev && ((uintptr_t)iq) % 16) return fail(ACB_ERR_ARG, "device input must be 16-byte aligned");
+	if (!dev && !c->d_iq[0]) return fail(ACB_ERR_ARG, "context created with ACB_FLAG_NO_INPUT_STAGING");
+	const int n = c->cfg.nstreams;
+	bool even = true;
+	for (int s = 0; nblk_s && s < n; s++) even = even && nblk_s[s] == nblk;
+	std::vector<size_t> rows(n, (size_t)nblk * OUTBLK), bytes(n, (size_t)nblk * c->blk_bytes);
+	for (int s = 0; !even && s < n; s++) rows[s] = (size_t)nblk_s[s] * OUTBLK, bytes[s] = (size_t)nblk_s[s] * c->blk_bytes;
+	int slot = -1;
+	if (!even) {
+		if (int r = stage_begin(c, slot)) return r;
+		for (int s = 0; s < n; s++) c->h_rag[slot][s] = (int)rows[s], c->h_rag[slot][n + s] = nblk_s[s];
+		if (int r = stage_upload(c, slot)) return r;
+	}
+	const int b = c->next_buf;
+	const size_t per_stream = (size_t)nblk * c->blk_bytes;
+	if (!dev) {
+		c->next_buf ^= 1;
+		/* the kernels that last read this staging buffer must be done before it is overwritten */
+		if (c->buf_used[b]) CU(cudaStreamWaitEvent(c->s_copy, c->ev_consumed[b], 0));
+		if (even && (stride == per_stream || n == 1)) {
+			CU(cudaMemcpyAsync(c->d_iq[b], iq, per_stream * n, cudaMemcpyHostToDevice, c->s_copy));
+		} else if (int r = copy_rows(c, c->d_iq[b], per_stream, iq, stride, bytes, 1, even)) {
+			return r;
+		}
+		CU(cudaEventRecord(c->ev_copied[b], c->s_copy));
+		CU(cudaStreamWaitEvent(c->s_comp, c->ev_copied[b], 0));
+	}
+	if (int r = run_kernels(c, dev ? iq : c->d_iq[b], dev ? stride : per_stream, nblk, nblk * OUTBLK, nullptr, submit_groups(c, rows),
+	                        even ? nullptr : c->d_rag[slot], even ? nullptr : c->h_rag[slot]))
+		return r;
+	if (!dev) {
+		CU(cudaEventRecord(c->ev_consumed[b], c->s_comp));      /* staging buffer is free once K1 has read it */
+		c->buf_used[b] = true;
+	}
+	if (!even)
+		if (int r = stage_end(c, slot)) return r;
+	for (int s = 0; s < n; s++) {
+		c->pos[s] += rows[s];
+		c->stats.blocks += rows[s] / OUTBLK;
+	}
+	return ACB_OK;
 }
 
 extern "C" int acb_submit_device(acb_ctx_t *c, const uint8_t *iq_dev, size_t stride, int nblk)
 {
 	if (int r = check_blocks(c, iq_dev, stride, nblk)) return r;
-	if (int r = ctx_use(c)) return r;
-	if (((uintptr_t)iq_dev) % 16) return fail(ACB_ERR_ARG, "device input must be 16-byte aligned");
-	if (int r = run_kernels(c, iq_dev, stride, nblk, nblk * OUTBLK, nullptr, block_groups(c, nblk))) return r;
-	c->pos += (unsigned long long)nblk * OUTBLK;
-	c->stats.blocks += (uint64_t)nblk * c->cfg.nstreams;
-	return ACB_OK;
+	return submit_blocks(c, iq_dev, stride, nblk, nullptr, true);
 }
 
 extern "C" int acb_submit_host(acb_ctx_t *c, const uint8_t *iq, size_t stride, int nblk)
 {
 	if (int r = check_blocks(c, iq, stride, nblk)) return r;
-	if (int r = ctx_use(c)) return r;
-	if (!c->d_iq[0]) return fail(ACB_ERR_ARG, "context created with ACB_FLAG_NO_INPUT_STAGING");
-	const int b = c->next_buf;
-	c->next_buf ^= 1;
-	const size_t per_stream = (size_t)nblk * c->blk_bytes;
-	/* the kernels that last read this staging buffer must be done before it is overwritten */
-	if (c->buf_used[b]) CU(cudaStreamWaitEvent(c->s_copy, c->ev_consumed[b], 0));
-	if (stride == per_stream || c->cfg.nstreams == 1) {
-		CU(cudaMemcpyAsync(c->d_iq[b], iq, per_stream * c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
-	} else {
-		CU(cudaMemcpy2DAsync(c->d_iq[b], per_stream, iq, stride, per_stream, c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
-	}
-	CU(cudaEventRecord(c->ev_copied[b], c->s_copy));
-	CU(cudaStreamWaitEvent(c->s_comp, c->ev_copied[b], 0));
-	if (int r = run_kernels(c, c->d_iq[b], per_stream, nblk, nblk * OUTBLK, nullptr, block_groups(c, nblk))) return r;
-	CU(cudaEventRecord(c->ev_consumed[b], c->s_comp));      /* staging buffer is free once K1 has read it */
-	c->buf_used[b] = true;
-	c->pos += (unsigned long long)nblk * OUTBLK;
-	c->stats.blocks += (uint64_t)nblk * c->cfg.nstreams;
-	return ACB_OK;
+	return submit_blocks(c, iq, stride, nblk, nullptr, false);
+}
+
+extern "C" int acb_submit_device_ragged(acb_ctx_t *c, const uint8_t *iq_dev, size_t stride, const int *nblk)
+{
+	int maxb = 0;
+	if (int r = check_blocks_ragged(c, iq_dev, stride, nblk, maxb)) return r;
+	return submit_blocks(c, iq_dev, stride, maxb, nblk, true);
+}
+
+extern "C" int acb_submit_host_ragged(acb_ctx_t *c, const uint8_t *iq, size_t stride, const int *nblk)
+{
+	int maxb = 0;
+	if (int r = check_blocks_ragged(c, iq, stride, nblk, maxb)) return r;
+	return submit_blocks(c, iq, stride, maxb, nblk, false);
 }
 
 extern "C" int acb_set_emission_groups(acb_ctx_t *c, int unit, uint64_t period)
@@ -1159,73 +1449,122 @@ std::vector<unsigned long long> acb::stream_groups(int unit, unsigned long long 
 /* 4-byte samples (float32 real or int16 I,Q) of arbitrary count: appended behind the carried
  * remainder in d_real[b]; `x2` != NULL means planar int16 input (x = I plane, x2 = Q plane), which
  * is interleaved on the way.  `dev`: the input is in device memory (the device calls) and one append
- * kernel moves it; otherwise strided host copies bring it over.  Everything else is the same for both. */
-static int submit4(acb_ctx *c, const void *x, const void *x2, bool dev, size_t stride_samples, size_t nsamples)
+ * kernel moves it; otherwise strided host copies bring it over.  Everything else is the same for both.
+ * `ns` != NULL (the ragged calls): stream s brings ns[s] samples and its rows go to nout[s] (may be NULL); streams whose
+ * counts and carries all agree take the lockstep path. */
+static int submit4(acb_ctx *c, const void *x, const void *x2, bool dev, size_t stride_samples, size_t nsamples,
+                   const size_t *ns = nullptr, size_t *nout_s = nullptr)
 {
 	if (int r = ctx_use(c)) return r;
-	const size_t K = (size_t)c->cfg.K, total = c->carry + nsamples, hp = (size_t)c->hpad;
-	const size_t nout = total / K;
-	if (nsamples == 0 || hp + total > c->real_cap || nout > (size_t)c->cfg.max_blocks * OUTBLK)
-		return fail(ACB_ERR_ARG, "nsamples=%zu exceeds max_blocks*1024*K", nsamples);
-	if (c->cfg.nstreams > 1 && stride_samples < nsamples) return fail(ACB_ERR_ARG, "stream stride smaller than one stream's input");
+	const int n = c->cfg.nstreams;
+	const size_t K = (size_t)c->cfg.K, hp = (size_t)c->hpad;
+	std::vector<size_t> cnt(n), rows(n), rem(n);
+	size_t nmax = 0, omax = 0;
+	bool even = true;
+	for (int s = 0; s < n; s++) {
+		cnt[s] = ns ? ns[s] : nsamples;
+		const size_t total = c->carry[s] + cnt[s];
+		rows[s] = total / K;
+		rem[s] = total - rows[s] * K;
+		if ((!ns && nsamples == 0) || hp + total > c->real_cap || rows[s] > (size_t)c->cfg.max_blocks * OUTBLK)
+			return ns ? fail(ACB_ERR_ARG, "nsamples[%d]=%zu exceeds max_blocks*1024*K", s, cnt[s])
+			          : fail(ACB_ERR_ARG, "nsamples=%zu exceeds max_blocks*1024*K", nsamples);
+		if (cnt[s] > (size_t)INT32_MAX) return fail(ACB_ERR_ARG, "nsamples[%d]=%zu exceeds 2^31 - 1", s, cnt[s]);
+		nmax = std::max(nmax, cnt[s]);
+		omax = std::max(omax, rows[s]);
+		even = even && cnt[s] == cnt[0] && c->carry[s] == c->carry[0];
+	}
+	if (nmax == 0) return fail(ACB_ERR_ARG, "every stream's nsamples is 0");
+	if (even) nsamples = cnt[0];              /* a ragged call with equal counts and carries is the lockstep call */
+	if (n > 1 && stride_samples < nmax) return fail(ACB_ERR_ARG, "stream stride smaller than one stream's input");
 	const int b = c->real_buf;
 	/* The copy runs on the copy stream, so the H2D of submit i+1 overlaps the channelizer of submit i.
 	 * d_real[b] was last read by the channelizer two submits ago and by the copy that moved its tail on.
 	 * taps > K: the first hp samples of each stream are its history, rows start behind them. */
 	float *const buf0 = c->d_real[b], *const buf = buf0 + hp;
+	int slot = -1;
+	const int *rag = nullptr;
+	if (!even) {
+		if (int r = stage_begin(c, slot)) return r;
+		int *h = c->h_rag[slot];
+		for (int s = 0; s < n; s++) h[s] = (int)rows[s], h[n + s] = (int)c->carry[s], h[2 * n + s] = (int)cnt[s], h[3 * n + s] = (int)rem[s];
+		rag = c->d_rag[slot];
+	}
 	if (c->real_used[b]) CU(cudaStreamWaitEvent(c->s_copy, c->ev_real_free[b], 0));
+	if (!even)
+		if (int r = stage_upload(c, slot)) return r;
+	uint32_t *const dst = reinterpret_cast<uint32_t *>(buf);
 	if (dev) {
 		/* acb_wait_event: the caller's producer must be done before the append reads the input */
 		if (c->order_pending) {
 			CU(cudaStreamWaitEvent(c->s_copy, c->ev_order, 0));
 			c->order_pending = false;
 		}
-		int r = launch_append4(x, x2, stride_samples, reinterpret_cast<uint32_t *>(buf + c->carry), c->real_cap, nsamples,
-		                       c->cfg.nstreams, c->s_copy);
+		int r = even ? launch_append4(x, x2, stride_samples, dst + c->carry[0], c->real_cap, nsamples, n, c->s_copy)
+		             : launch_append4_ragged(x, x2, stride_samples, dst, c->real_cap, rag + n, rag + 2 * n, nmax, n, c->s_copy);
 		if (r) return fail(ACB_ERR_CUDA, "append launch: %s", cudaGetErrorString((cudaError_t)r));
 		c->stats.kernel_launches++;
-	} else if (!x2) {
-		CU(cudaMemcpy2DAsync(buf + c->carry, c->real_cap * sizeof(float), x, stride_samples * sizeof(float),
-		                     nsamples * sizeof(float), c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
+	} else if (!x2 && even) {
+		CU(cudaMemcpy2DAsync(buf + c->carry[0], c->real_cap * sizeof(float), x, stride_samples * sizeof(float),
+		                     nsamples * sizeof(float), n, cudaMemcpyHostToDevice, c->s_copy));
 	} else {
 		/* planar int16 (the SDRplay callback's xi / xq): both planes go over as they are (two dense copies),
-		 * a small kernel interleaves them behind the carried remainder */
-		if (nsamples > c->planar_cap) {
+		 * a small kernel interleaves them behind the carried remainder.  Ragged interleaved input goes over the same
+		 * way, as 4-byte samples, and the ragged append puts each stream behind its own carry. */
+		if (nmax > c->planar_cap) {
 			CU(cudaStreamSynchronize(c->s_copy));
 			cudaFree(c->d_planar);
 			c->d_planar = nullptr;
-			c->planar_cap = std::max(nsamples, (size_t)c->cfg.max_blocks * OUTBLK * K);
-			CU(cudaMalloc(&c->d_planar, 2 * (size_t)c->cfg.nstreams * c->planar_cap * sizeof(int16_t)));
+			c->planar_cap = std::max(nmax, (size_t)c->cfg.max_blocks * OUTBLK * K);
+			CU(cudaMalloc(&c->d_planar, 2 * (size_t)n * c->planar_cap * sizeof(int16_t)));
 		}
-		int16_t *pi = c->d_planar, *pq = c->d_planar + (size_t)c->cfg.nstreams * c->planar_cap;
-		CU(cudaMemcpy2DAsync(pi, c->planar_cap * 2, x, stride_samples * 2, nsamples * 2, c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
-		CU(cudaMemcpy2DAsync(pq, c->planar_cap * 2, x2, stride_samples * 2, nsamples * 2, c->cfg.nstreams, cudaMemcpyHostToDevice, c->s_copy));
-		int r = launch_interleave_cs16(pi, pq, c->planar_cap, reinterpret_cast<uint32_t *>(buf + c->carry), c->real_cap, nsamples, c->cfg.nstreams, c->s_copy);
+		int r = 0;
+		if (!x2) {
+			uint32_t *stg = reinterpret_cast<uint32_t *>(c->d_planar);
+			if (int e = copy_rows(c, stg, c->planar_cap * 4, x, stride_samples * 4, cnt, 4, false)) return e;
+			r = launch_append4_ragged(stg, nullptr, c->planar_cap, dst, c->real_cap, rag + n, rag + 2 * n, nmax, n, c->s_copy);
+		} else {
+			int16_t *pi = c->d_planar, *pq = c->d_planar + (size_t)n * c->planar_cap;
+			if (int e = copy_rows(c, pi, c->planar_cap * 2, x, stride_samples * 2, cnt, 2, even)) return e;
+			if (int e = copy_rows(c, pq, c->planar_cap * 2, x2, stride_samples * 2, cnt, 2, even)) return e;
+			r = even ? launch_interleave_cs16(pi, pq, c->planar_cap, dst + c->carry[0], c->real_cap, nsamples, n, c->s_copy)
+			         : launch_append4_ragged(pi, pq, c->planar_cap, dst, c->real_cap, rag + n, rag + 2 * n, nmax, n, c->s_copy);
+		}
 		if (r) return fail(ACB_ERR_CUDA, "interleave launch: %s", cudaGetErrorString((cudaError_t)r));
 		c->stats.kernel_launches++;
 	}
 	CU(cudaEventRecord(c->ev_real_copied, c->s_copy));
 	CU(cudaStreamWaitEvent(c->s_comp, c->ev_real_copied, 0));
-	const size_t rem = total - nout * K;
-	if (nout) {
-		if (int r = run_kernels(c, (const uint8_t *)buf, c->real_cap * sizeof(float), 0, (int)nout, nullptr,
-		                        stream_groups(c->group_unit, c->group_period, c->cfg.K, c->pos, nout)))
+	if (omax) {
+		if (int r = run_kernels(c, (const uint8_t *)buf, c->real_cap * sizeof(float), 0, (int)omax, nullptr, submit_groups(c, rows), rag,
+		                        even ? nullptr : c->h_rag[slot]))
 			return r;
-		c->pos += nout;
 		/* the unconsumed tail (air.c:329-334 / soapy.c:238-252 keep a partial sum instead: same
 		 * arithmetic order) moves to the front of the other buffer, behind the hp samples before it (the next
 		 * submit's history, taps > K) */
-		if (rem + hp) {
+		if (even && rem[0] + hp) {
 			if (c->real_used[b ^ 1]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_real_free[b ^ 1], 0));
-			CU(cudaMemcpy2DAsync(c->d_real[b ^ 1], c->real_cap * sizeof(float), buf + nout * K - hp, c->real_cap * sizeof(float),
-			                     (hp + rem) * sizeof(float), c->cfg.nstreams, cudaMemcpyDeviceToDevice, c->s_comp));
+			CU(cudaMemcpy2DAsync(c->d_real[b ^ 1], c->real_cap * sizeof(float), buf + omax * K - hp, c->real_cap * sizeof(float),
+			                     (hp + rem[0]) * sizeof(float), n, cudaMemcpyDeviceToDevice, c->s_comp));
+		} else if (!even) {
+			if (c->real_used[b ^ 1]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_real_free[b ^ 1], 0));
+			int r = launch_move_tail(reinterpret_cast<const uint32_t *>(buf0), reinterpret_cast<uint32_t *>(c->d_real[b ^ 1]), c->real_cap,
+			                         c->cfg.K, c->hpad, rag, rag + 3 * n, n, c->s_comp);
+			if (r) return fail(ACB_ERR_CUDA, "tail move launch: %s", cudaGetErrorString((cudaError_t)r));
+			c->stats.kernel_launches++;
 		}
 		CU(cudaEventRecord(c->ev_real_free[b], c->s_comp));
 		c->real_used[b] = true;
 		c->real_buf = b ^ 1;
 	}
-	c->carry = rem;          /* nout == 0: the samples simply stay behind the previous carry */
-	return (int)nout;
+	if (!even)
+		if (int r = stage_end(c, slot)) return r;
+	for (int s = 0; s < n; s++) {
+		c->pos[s] += rows[s];
+		c->carry[s] = rem[s];          /* no row: the samples simply stay behind the previous carry */
+		if (nout_s) nout_s[s] = rows[s];
+	}
+	return (int)omax;
 }
 
 extern "C" int acb_submit_real_host(acb_ctx_t *c, const float *x, size_t stride_samples, size_t nsamples)
@@ -1291,6 +1630,56 @@ extern "C" int acb_submit_cs16_planar_device(acb_ctx_t *c, const int16_t *xi_dev
 	return submit4(c, xi_dev, xq_dev, true, stride_samples, nsamples);
 }
 
+/* the ragged forms: the same calls with a count per stream */
+extern "C" int acb_submit_real_host_ragged(acb_ctx_t *c, const float *x, size_t stride_samples, const size_t *nsamples, size_t *nout)
+{
+	if (!c || !x || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_F32REAL) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_REAL_INPUT");
+	return submit4(c, x, nullptr, false, stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_submit_cs16_host_ragged(acb_ctx_t *c, const int16_t *iq, size_t stride_samples, const size_t *nsamples, size_t *nout)
+{
+	if (!c || !iq || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	return submit4(c, iq, nullptr, false, stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_submit_cs16_planar_host_ragged(acb_ctx_t *c, const int16_t *xi, const int16_t *xq, size_t stride_samples,
+                                                  const size_t *nsamples, size_t *nout)
+{
+	if (!c || !xi || !xq || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	return submit4(c, xi, xq, false, stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_submit_real_device_ragged(acb_ctx_t *c, const float *x_dev, size_t stride_samples, const size_t *nsamples, size_t *nout)
+{
+	if (!c || !x_dev || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_F32REAL) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_REAL_INPUT");
+	if (int r = check_device_input(c, x_dev, 4)) return r;
+	return submit4(c, x_dev, nullptr, true, stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_submit_cs16_device_ragged(acb_ctx_t *c, const int16_t *iq_dev, size_t stride_samples, const size_t *nsamples,
+                                             size_t *nout)
+{
+	if (!c || !iq_dev || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	if (int r = check_device_input(c, iq_dev, 4)) return r;
+	return submit4(c, iq_dev, nullptr, true, stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_submit_cs16_planar_device_ragged(acb_ctx_t *c, const int16_t *xi_dev, const int16_t *xq_dev, size_t stride_samples,
+                                                    const size_t *nsamples, size_t *nout)
+{
+	if (!c || !xi_dev || !xq_dev || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	if (c->in_kind != IN_KIND_CS16IQ) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_CS16_INPUT");
+	if (int r = check_device_input(c, xi_dev, 2)) return r;
+	if (int r = check_device_input(c, xq_dev, 2)) return r;
+	return submit4(c, xi_dev, xq_dev, true, stride_samples, 0, nsamples, nout);
+}
+
 extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, int variant, unsigned fc_hz, unsigned *fc_out)
 {
 	if (!c || !freqs_hz) return fail(ACB_ERR_ARG, "null argument");
@@ -1351,8 +1740,10 @@ extern "C" int acb_submit_dm_host(acb_ctx_t *c, const float *dm, int nsamp)
 	if (nsamp < 1 || n > c->dm_floats) return fail(ACB_ERR_ARG, "nsamp=%d exceeds max_blocks*1024", nsamp);
 	/* A pageable source has been staged when the call returns; a pinned one must stay untouched
 	 * until the submit is collected. */
-	if (int r = run_kernels(c, nullptr, 0, 0, nsamp, dm, std::vector<unsigned long long>{ c->pos })) return r;
-	c->pos += (unsigned long long)nsamp;
+	Groups g;
+	g.starts.push_back(*std::min_element(c->pos.begin(), c->pos.end()));
+	if (int r = run_kernels(c, nullptr, 0, 0, nsamp, dm, std::move(g))) return r;
+	for (auto &p : c->pos) p += (unsigned long long)nsamp;
 	return ACB_OK;
 }
 

@@ -222,7 +222,7 @@ template <bool F2F> ACB_HD int bit_clock_fire(const DcConsts &DCK_, double &clkd
  * registers and only differ in which mixer evaluations they contribute.  Env supplies the warp
  * collectives (identity on the host).  FrameAcc is frame_sm.h's accessor over `r`; it reads r.pos0 +
  * r.fire_n when it needs a sample position. */
-template <int L, bool F2F, bool PIN, class Env, class FrameAcc, int CPW>
+template <int L, bool F2F, bool PIN, class Env, bool RAGGED = false, class FrameAcc, int CPW>
 ACB_HD void demod_run(DemodRegs &r, DemodShared<CPW> &sm, const float *in, int nch, int nsamp, int sub, int grp,
                       FrameAcc &acc)
 {
@@ -268,7 +268,11 @@ DC_UNROLL
 	for (;;) {
 		if (budget == 0) {
 			if (!Env::any(n < nsamp)) break;
-			budget = (nsamp - Env::max(n)) / DEMOD_LOOK;
+			/* RAGGED: the groups of a warp have different sample counts, so the budget must still be the same for the whole
+			 * warp; any budget >= 1 is correct (a group that runs out idles through the general path), the largest
+			 * remaining count keeps the votes as rare as in the even case */
+			if constexpr (RAGGED) budget = Env::max(nsamp - n) / DEMOD_LOOK;
+			else budget = (nsamp - Env::max(n)) / DEMOD_LOOK;
 			if (budget < 1) budget = 1;
 		}
 		budget--;

@@ -2456,9 +2456,8 @@ int launch_interleave_cs16(const int16_t *xi, const int16_t *xq, size_t plane_st
  * row starts at hpad + carry samples, generally not on 16 bytes, so a head of up to 3 samples and a tail of up to 3 go
  * singly and every whole 16-byte unit between them is one vector store.  Pure data movement, read once, written once. */
 template <bool PLANAR>
-__global__ void __launch_bounds__(256)
-k_append4(const void *__restrict__ a, const void *__restrict__ b, size_t src_stride, uint32_t *__restrict__ out,
-          size_t out_stride, size_t nsamples)
+__device__ __forceinline__ void append4_row(const void *__restrict__ a, const void *__restrict__ b, size_t src_stride,
+                                            uint32_t *__restrict__ out, size_t out_stride, size_t nsamples)
 {
 	const int s = blockIdx.y;
 	const uint32_t *x = reinterpret_cast<const uint32_t *>(a) + (size_t)s * src_stride;
@@ -2479,6 +2478,75 @@ k_append4(const void *__restrict__ a, const void *__restrict__ b, size_t src_str
 	}
 	if (tid < head) o[tid] = at(tid);
 	if (tid < nsamples - tail0) o[tail0 + tid] = at(tail0 + tid);
+}
+
+template <bool PLANAR>
+__global__ void __launch_bounds__(256)
+k_append4(const void *__restrict__ a, const void *__restrict__ b, size_t src_stride, uint32_t *__restrict__ out,
+          size_t out_stride, size_t nsamples)
+{
+	append4_row<PLANAR>(a, b, src_stride, out, out_stride, nsamples);
+}
+
+/* The ragged form: stream s's count[s] samples land at out + s*out_stride + off[s] (its history and own carry) */
+template <bool PLANAR>
+__global__ void __launch_bounds__(256)
+k_append4_ragged(const void *__restrict__ a, const void *__restrict__ b, size_t src_stride, uint32_t *__restrict__ out,
+                 size_t out_stride, const int *__restrict__ off, const int *__restrict__ count)
+{
+	const int s = blockIdx.y;
+	append4_row<PLANAR>(a, b, src_stride, out + off[s], out_stride, (size_t)count[s]);
+}
+
+int launch_append4_ragged(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, const int *off,
+                          const int *count, size_t max_count, int nstreams, cudaStream_t stream)
+{
+	if (max_count == 0) return 0;
+	const unsigned gx = (unsigned)std::min<size_t>((max_count / 4 + 255) / 256 + 1, 1184);
+	if (b) k_append4_ragged<true><<<dim3(gx, nstreams), 256, 0, stream>>>(a, b, src_stride, out, out_stride, off, count);
+	else k_append4_ragged<false><<<dim3(gx, nstreams), 256, 0, stream>>>(a, nullptr, src_stride, out, out_stride, off, count);
+	return (int)cudaGetLastError();
+}
+
+/* Ragged streaming submits: stream s's unconsumed tail (its last `hpad` samples before it, the next submit's history, and
+ * rem[s] samples no row took) moves from src + s*stride + nrows[s]*K to the front of the other buffer, dst + s*stride */
+__global__ void __launch_bounds__(256)
+k_move_tail(const uint32_t *__restrict__ src, uint32_t *__restrict__ dst, size_t stride, int K, int hpad,
+            const int *__restrict__ nrows, const int *__restrict__ rem)
+{
+	const int s = blockIdx.y;
+	const uint32_t *p = src + (size_t)s * stride + (size_t)nrows[s] * K;
+	uint32_t *o = dst + (size_t)s * stride;
+	const int n = hpad + rem[s];
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) o[i] = p[i];
+}
+
+int launch_move_tail(const uint32_t *src, uint32_t *dst, size_t stride, int K, int hpad, const int *nrows, const int *rem,
+                     int nstreams, cudaStream_t stream)
+{
+	const unsigned gx = (unsigned)((hpad + K + 255) / 256);      /* rem < K */
+	k_move_tail<<<dim3(gx, nstreams), 256, 0, stream>>>(src, dst, stride, K, hpad, nrows, rem);
+	return (int)cudaGetLastError();
+}
+
+/* Ragged u8 submits at taps > K: stream s's last `hb` bytes of input, at in + s*stride + nblk[s]*blk_bytes - hb, become its
+ * history; a stream that brought no block keeps the history it had */
+__global__ void __launch_bounds__(256)
+k_hist_gather(const uint8_t *__restrict__ in, size_t stride, size_t blk_bytes, const int *__restrict__ nblk,
+              uint8_t *__restrict__ hist, int hb)
+{
+	const int s = blockIdx.y;
+	if (nblk[s] == 0) return;
+	const uint8_t *p = in + (size_t)s * stride + (size_t)nblk[s] * blk_bytes - hb;
+	uint8_t *o = hist + (size_t)s * hb;
+	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < hb; i += gridDim.x * blockDim.x) o[i] = p[i];
+}
+
+int launch_hist_gather(const uint8_t *in, size_t stride, size_t blk_bytes, const int *nblk, uint8_t *hist, int hb, int nstreams,
+                       cudaStream_t stream)
+{
+	k_hist_gather<<<dim3((unsigned)((hb + 255) / 256), nstreams), 256, 0, stream>>>(in, stride, blk_bytes, nblk, hist, hb);
+	return (int)cudaGetLastError();
 }
 
 int launch_append4(const void *a, const void *b, size_t src_stride, uint32_t *out, size_t out_stride, size_t nsamples, int nstreams,
@@ -3013,10 +3081,11 @@ int upload_matched_filter(const float *h, cudaStream_t stream)
 
 /* K2's body, shared by k_demod2 and its counting form k_demod2_stats (STATS: the frame synchroniser's events go to
  * counts[chain * EV_COUNT + e]; k_demod2 passes none and never sees the hook) */
-template <int L, bool F2F, bool PIN, bool STATS>
+template <int L, bool F2F, bool PIN, bool STATS, bool RAGGED = false>
 __device__ __forceinline__ void demod2_body(DemodShared<32 / L> &sm, ChainState *__restrict__ states, const float *__restrict__ dm,
                                             int nsamp, int nch, int nstreams, RawFrame *__restrict__ ring,
-                                            RingCtl *__restrict__ ctl, unsigned cap, unsigned *__restrict__ counts)
+                                            RingCtl *__restrict__ ctl, unsigned cap, unsigned *__restrict__ counts,
+                                            const int *__restrict__ nrows = nullptr)
 {
 	constexpr int CPW = 32 / L;                  /* channels per warp */
 	const int lane = threadIdx.x;
@@ -3049,12 +3118,14 @@ __device__ __forceinline__ void demod2_body(DemodShared<32 / L> &sm, ChainState 
 	}
 	__syncwarp();
 
+	/* RAGGED: stream s has nrows[s] rows of its own; the envelope keeps the launch's nsamp rows per stream */
+	const int n_s = RAGGED ? nrows[s] : nsamp;
 	if constexpr (STATS) {
 		DevFrameAccStats acc{ { r, st, ring, ctl, cap, s, ch, leader, true }, counts + (size_t)g * EV_COUNT };
-		demod_run<L, F2F, PIN, WarpEnv>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, nsamp, sub, grp, acc);
+		demod_run<L, F2F, PIN, WarpEnv, RAGGED>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, n_s, sub, grp, acc);
 	} else {
 		DevFrameAcc acc{ r, st, ring, ctl, cap, s, ch, leader, true };
-		demod_run<L, F2F, PIN, WarpEnv>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, nsamp, sub, grp, acc);
+		demod_run<L, F2F, PIN, WarpEnv, RAGGED>(r, sm, dm + (size_t)s * nsamp * nch + ch, nch, n_s, sub, grp, acc);
 	}
 
 	if (!leader) return;
@@ -3083,6 +3154,27 @@ k_demod2_stats(ChainState *__restrict__ states, const float *__restrict__ dm, in
 {
 	__shared__ DemodShared<32 / L> sm;
 	demod2_body<L, F2F, PIN, true>(sm, states, dm, nsamp, nch, nstreams, ring, ctl, cap, counts);
+}
+
+/* The ragged forms (submits whose streams carry different row counts): stream s demodulates nrows[s] of the nsamp rows
+ * each stream has in the envelope; the same launch geometry, launch bounds and shared memory as the even forms */
+template <int L, bool F2F, bool PIN, int MINB = 1>
+__global__ void __launch_bounds__(32, MINB)
+k_demod2_ragged(ChainState *__restrict__ states, const float *__restrict__ dm, int nsamp, int nch, int nstreams,
+                RawFrame *__restrict__ ring, RingCtl *__restrict__ ctl, unsigned cap, const int *__restrict__ nrows)
+{
+	__shared__ DemodShared<32 / L> sm;
+	demod2_body<L, F2F, PIN, false, true>(sm, states, dm, nsamp, nch, nstreams, ring, ctl, cap, nullptr, nrows);
+}
+
+template <int L, bool F2F, bool PIN, int MINB = 1>
+__global__ void __launch_bounds__(32, MINB)
+k_demod2_stats_ragged(ChainState *__restrict__ states, const float *__restrict__ dm, int nsamp, int nch, int nstreams,
+                      RawFrame *__restrict__ ring, RingCtl *__restrict__ ctl, unsigned cap, unsigned *__restrict__ counts,
+                      const int *__restrict__ nrows)
+{
+	__shared__ DemodShared<32 / L> sm;
+	demod2_body<L, F2F, PIN, true, true>(sm, states, dm, nsamp, nch, nstreams, ring, ctl, cap, counts, nrows);
 }
 
 /* SM count and shared memory per SM of the current device, asked per launch: contexts of one process may sit on
@@ -3119,9 +3211,10 @@ constexpr int DEMOD_SMEM_BESIDE = 3 * (4096 + DEMOD_SMEM_RESERVED);   /* three k
 constexpr int DEMOD_MAX_WARPS_PER_SM = 16;
 constexpr int DEMOD_MIN_WARPS_SHARING = 4;                      /* per SM: below, K2 is the step and keeps the largest carve-out */
 
-template <int LANES, bool F2F, bool PIN, int MINB = 1, bool STATS = false>
+template <int LANES, bool F2F, bool PIN, int MINB = 1, bool STATS = false, bool RAGGED = false>
 static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                          RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
+                          RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr,
+                          const int *nrows = nullptr)
 {
 	constexpr int CPW = 32 / LANES;
 	const int wps = (nch + CPW - 1) / CPW;
@@ -3133,6 +3226,17 @@ static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, i
 	const long long need = per_sm * ((long long)sizeof(DemodShared<CPW>) + DEMOD_SMEM_RESERVED) + DEMOD_SMEM_BESIDE;
 	const int carve = per_sm < DEMOD_MIN_WARPS_SHARING ? (int)cudaSharedmemCarveoutMaxShared
 	                                                   : (int)std::min<long long>(100, (need * 100 + smem_per_sm - 1) / smem_per_sm);
+	if constexpr (RAGGED && STATS) {
+		cudaError_t e = cudaFuncSetAttribute(k_demod2_stats_ragged<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
+		if (e != cudaSuccess) return (int)e;
+		k_demod2_stats_ragged<LANES, F2F, PIN, MINB><<<grid, 32, 0, stream>>>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, counts, nrows);
+		return (int)cudaGetLastError();
+	} else if constexpr (RAGGED) {
+		cudaError_t e = cudaFuncSetAttribute(k_demod2_ragged<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
+		if (e != cudaSuccess) return (int)e;
+		k_demod2_ragged<LANES, F2F, PIN, MINB><<<grid, 32, 0, stream>>>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, nrows);
+		return (int)cudaGetLastError();
+	}
 	if constexpr (STATS) {
 		cudaError_t e = cudaFuncSetAttribute(k_demod2_stats<LANES, F2F, PIN, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout, carve);
 		if (e != cudaSuccess) return (int)e;
@@ -3149,15 +3253,17 @@ static int launch_demod_t(ChainState *st, const float *dm, int nsamp, int nch, i
  * (__launch_bounds__(32, 1)), ptxas spends more registers on a wider schedule: fewer instructions where the kernel is
  * latency bound, but fewer warps per SM where it is not.  So: the wide schedule while there are at most 8 warps per SM,
  * the lean one beyond. */
-template <int LANES, bool F2F, bool STATS = false>
+template <int LANES, bool F2F, bool STATS = false, bool RAGGED = false>
 static int launch_demod_pinned(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                               RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
+                               RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr,
+                               const int *nrows = nullptr)
 {
 	int sm_count, smem_per_sm;
 	demod_sm_limits(sm_count, smem_per_sm);
 	const long long warps = ((long long)nstreams * nch * LANES + 31) / 32;
-	return warps <= 8LL * sm_count ? launch_demod_t<LANES, F2F, true, 1, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts)
-	                               : launch_demod_t<LANES, F2F, true, 0, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts);
+	return warps <= 8LL * sm_count
+	           ? launch_demod_t<LANES, F2F, true, 1, STATS, RAGGED>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts, nrows)
+	           : launch_demod_t<LANES, F2F, true, 0, STATS, RAGGED>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts, nrows);
 }
 
 /* The one-lane form in two register budgets.  Left alone ptxas takes 128 registers per thread; of those CTAs six fit
@@ -3168,16 +3274,18 @@ static int launch_demod_pinned(ChainState *st, const float *dm, int nsamp, int n
 constexpr int DEMOD_MINB_96REG = 20;
 constexpr int DEMOD_WARPS_PER_K1_CTA = 6;
 
-template <bool STATS = false>
+template <bool STATS = false, bool RAGGED = false>
 static int launch_demod_one_lane(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                                 RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr)
+                                 RawFrame *ring, RingCtl *ctl, unsigned cap, cudaStream_t stream, unsigned *counts = nullptr,
+                                 const int *nrows = nullptr)
 {
 	int sm_count, smem_per_sm;
 	demod_sm_limits(sm_count, smem_per_sm);
 	const long long warps = ((long long)nstreams * nch + 31) / 32;
 	return warps <= (long long)DEMOD_WARPS_PER_K1_CTA * sm_count
-	           ? launch_demod_t<1, false, false, 1, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts)
-	           : launch_demod_t<1, false, false, DEMOD_MINB_96REG, STATS>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts);
+	           ? launch_demod_t<1, false, false, 1, STATS, RAGGED>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts, nrows)
+	           : launch_demod_t<1, false, false, DEMOD_MINB_96REG, STATS, RAGGED>(st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts,
+	                                                                              nrows);
 }
 
 template <int LANES>
@@ -3211,8 +3319,19 @@ int demod_pick_lanes(long long nchains, int sm_count)
  * with the F2F conversion pair instead of integer ops (round_to_f32); negative (-4, -8) = the round-1 kernel, kept for
  * A/B runs */
 int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                 RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes, cudaStream_t stream)
+                 RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes, cudaStream_t stream, const int *nrows)
 {
+	if (nrows) {                 /* the ragged forms of the default widths only */
+#define ACB_DEMOD_ARGS st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, nullptr, nrows
+		switch (lanes) {
+		case 8: return launch_demod_pinned<8, false, false, true>(ACB_DEMOD_ARGS);
+		case 4: return launch_demod_pinned<4, false, false, true>(ACB_DEMOD_ARGS);
+		case 2: return launch_demod_pinned<2, false, false, true>(ACB_DEMOD_ARGS);
+		case 1: return launch_demod_one_lane<false, true>(ACB_DEMOD_ARGS);
+		default: return (int)cudaErrorInvalidValue;
+		}
+#undef ACB_DEMOD_ARGS
+	}
 #define ACB_DEMOD_ARGS st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream
 	switch (lanes) {
 	case -8: return launch_demod_v1<8>(ACB_DEMOD_ARGS);
@@ -3235,8 +3354,19 @@ int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstrea
 /* the counting forms of the default widths (what launch_demod runs for lanes 1, 2, 4, 8), each in the same register
  * budgets and under the same carve-out rules */
 int launch_demod_stats(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
-                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes, unsigned *counts, cudaStream_t stream)
+                       RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes, unsigned *counts, cudaStream_t stream, const int *nrows)
 {
+	if (nrows) {
+#define ACB_DEMOD_ARGS st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts, nrows
+		switch (lanes) {
+		case 8: return launch_demod_pinned<8, false, true, true>(ACB_DEMOD_ARGS);
+		case 4: return launch_demod_pinned<4, false, true, true>(ACB_DEMOD_ARGS);
+		case 2: return launch_demod_pinned<2, false, true, true>(ACB_DEMOD_ARGS);
+		case 1: return launch_demod_one_lane<true, true>(ACB_DEMOD_ARGS);
+		default: return (int)cudaErrorInvalidValue;
+		}
+#undef ACB_DEMOD_ARGS
+	}
 #define ACB_DEMOD_ARGS st, dm, nsamp, nch, nstreams, ring, ctl, cap, stream, counts
 	switch (lanes) {
 	case 8: return launch_demod_pinned<8, false, true>(ACB_DEMOD_ARGS);

@@ -4,8 +4,9 @@
  * (SURVEY.md §8e: channels share nothing but the read-only matched filter, streams share nothing).
  * The reference has no counterpart (one thread serves all channels, rtl.c:344-360); what it fixes for us is the
  * emission order the merged output must keep: u8 IQ per 1024-sample block, then channel, then time (rtl.c:357-360);
- * the streaming front-ends (real input, CS16) per emission group of acb_set_emission_groups, which this layer keeps
- * track of itself because a message does not say which group it belongs to.
+ * the streaming front-ends (real input, CS16) per emission group of acb_set_emission_groups.  Every context orders
+ * each submit's frames by (group number counted from the stream's start, stream, channel, time); this layer keeps each
+ * stream's position after every submit not yet collected, because a message does not say which submit it came from.
  */
 #include <stdio.h>
 #include <string.h>
@@ -32,13 +33,13 @@ struct acb_multi {
 	std::vector<Part> parts;
 	std::deque<acb_msg_t> outq;
 	std::vector<acb_msg_t> scratch;
-	/* streaming kinds: the emission groups of the submits not yet collected, as every part's context cuts them
-	 * (acb::stream_groups); group starts only grow, so a message's group is the last start at or before its pos */
 	int group_unit;
 	unsigned long long group_period;
-	unsigned long long pos;            /* envelope samples submitted so far, per stream (the parts move together) */
-	std::deque<unsigned long long> gstarts;
-	std::deque<size_t> gcount;         /* starts per submit in flight, oldest first */
+	std::vector<unsigned long long> spos;   /* per (global) stream: envelope rows since create / reset */
+	/* the submits not yet collected, oldest first: each stream's position after it (a message belongs to the first
+	 * submit whose end lies beyond its pos) and which parts ran it (acb_multi_collect collects those) */
+	struct Sub { std::vector<unsigned long long> end; std::vector<unsigned char> part; };
+	std::deque<Sub> subs;
 };
 
 static void split(int n, int parts, int i, int *lo, int *cnt)
@@ -58,7 +59,7 @@ extern "C" int acb_multi_create(const acb_config_t *cfg, const int *devices, int
 	m->streaming = (cfg->flags & (ACB_FLAG_REAL_INPUT | ACB_FLAG_CS16_INPUT)) != 0;
 	m->group_unit = ACB_GROUP_SUBMIT;
 	m->group_period = 0;
-	m->pos = 0;
+	m->spos.assign(cfg->nstreams > 0 ? cfg->nstreams : 0, 0);
 	*out = m;
 	const int total = mode == ACB_MULTI_SPLIT_STREAMS ? cfg->nstreams : cfg->nch;
 	for (int i = 0; i < ndev; i++) {
@@ -153,10 +154,16 @@ extern "C" int acb_multi_reset(acb_multi_t *m)
 	for (auto &p : m->parts)
 		if (int r = acb_reset(p.ctx)) return r;
 	m->outq.clear();
-	m->pos = 0;
-	m->gstarts.clear();
-	m->gcount.clear();
+	std::fill(m->spos.begin(), m->spos.end(), 0);
+	m->subs.clear();
 	return ACB_OK;
+}
+
+/* A submit went to the parts marked in `ran`: stream s advanced by rows[s] */
+static void record_submit(acb_multi *m, const std::vector<size_t> &rows, std::vector<unsigned char> &&ran)
+{
+	for (size_t s = 0; s < rows.size(); s++) m->spos[s] += rows[s];
+	m->subs.push_back(acb_multi::Sub{ m->spos, std::move(ran) });
 }
 
 extern "C" int acb_multi_set_emission_groups(acb_multi_t *m, int unit, uint64_t period)
@@ -176,35 +183,87 @@ extern "C" int acb_multi_submit_host(acb_multi_t *m, const uint8_t *iq, size_t s
 	/* asynchronous per device (pinned source): every GPU pulls its part over its own PCIe link at once */
 	for (auto &p : m->parts)
 		if (int r = acb_submit_host(p.ctx, iq + (size_t)p.s0 * stream_stride, stream_stride, nblk)) return r;
+	record_submit(m, std::vector<size_t>(m->cfg.nstreams, (size_t)nblk * ACB_OUTBLK), std::vector<unsigned char>(m->parts.size(), 1));
+	return ACB_OK;
+}
+
+/* Ragged u8: a stream split hands each part its streams' counts (a part whose counts are all 0 sits the submit out), a
+ * channel split hands every part all of them.  The counts are checked here, before any part reads anything. */
+extern "C" int acb_multi_submit_host_ragged(acb_multi_t *m, const uint8_t *iq, size_t stream_stride, const int *nblk)
+{
+	if (!m || !iq || !nblk) return fail(ACB_ERR_ARG, "null argument");
+	if (m->streaming) return fail(ACB_ERR_ARG, "not a u8-IQ multi-context: use acb_multi_submit_real_host_ragged / acb_multi_submit_cs16_host_ragged");
+	const int n = m->cfg.nstreams;
+	int maxb = 0;
+	for (int s = 0; s < n; s++) {
+		if (nblk[s] < 0 || nblk[s] > m->cfg.max_blocks) return fail(ACB_ERR_ARG, "nblk[%d]=%d outside 0..%d", s, nblk[s], m->cfg.max_blocks);
+		maxb = std::max(maxb, nblk[s]);
+	}
+	if (maxb == 0) return fail(ACB_ERR_ARG, "every stream's nblk is 0");
+	if (n > 1 && stream_stride < (size_t)maxb * ACB_OUTBLK * m->cfg.K * 2) return fail(ACB_ERR_ARG, "stream_stride smaller than the largest input");
+	if (stream_stride % 16) return fail(ACB_ERR_ARG, "stream_stride must be a multiple of 16 bytes");
+	std::vector<unsigned char> ran(m->parts.size(), 0);
+	for (size_t i = 0; i < m->parts.size(); i++) {
+		const Part &p = m->parts[i];
+		if (std::all_of(nblk + p.s0, nblk + p.s0 + p.ns, [](int b) { return b == 0; })) continue;
+		if (int r = acb_submit_host_ragged(p.ctx, iq + (size_t)p.s0 * stream_stride, stream_stride, nblk + p.s0)) return r;
+		ran[i] = 1;
+	}
+	std::vector<size_t> rows(n);
+	for (int s = 0; s < n; s++) rows[s] = (size_t)nblk[s] * ACB_OUTBLK;
+	record_submit(m, rows, std::move(ran));
 	return ACB_OK;
 }
 
 /* The streaming submits: every part gets its streams' rows (stream split) or the whole input (channel split), each
- * pulling it over its own link.  Every part carries the same remainder, so all must produce the same rows. */
-static int submit_streaming(acb_multi *m, int flag, const void *x, const void *x2, size_t sample_bytes, size_t stride, size_t nsamples)
+ * pulling it over its own link.  In a channel split every part carries the same remainders, so all must produce the same
+ * rows.  `ns` != NULL: the ragged calls, stream s bringing ns[s] samples; a stream-split part whose counts are all 0 sits
+ * the submit out.  The lockstep calls return the rows every stream produced, the ragged ones the largest and nout[s]. */
+static int submit_streaming(acb_multi *m, int flag, const void *x, const void *x2, size_t sample_bytes, size_t stride, size_t nsamples,
+                            const size_t *ns = nullptr, size_t *nout_s = nullptr)
 {
 	if (!(m->cfg.flags & flag))
 		return fail(ACB_ERR_ARG, flag == ACB_FLAG_REAL_INPUT ? "multi-context was not created with ACB_FLAG_REAL_INPUT"
 		                                                     : "multi-context was not created with ACB_FLAG_CS16_INPUT");
+	const int n = m->cfg.nstreams;
+	size_t nmax = ns ? 0 : nsamples;
+	for (int s = 0; ns && s < n; s++) nmax = std::max(nmax, ns[s]);
+	if (ns && nmax == 0) return fail(ACB_ERR_ARG, "every stream's nsamples is 0");
 	/* a part with one stream does not check this itself */
-	if (m->cfg.nstreams > 1 && stride < nsamples) return fail(ACB_ERR_ARG, "stream stride smaller than one stream's input");
+	if (n > 1 && stride < nmax) return fail(ACB_ERR_ARG, "stream stride smaller than one stream's input");
+	std::vector<size_t> rows(n, 0), got(n, 0);
+	std::vector<unsigned char> ran(m->parts.size(), 0);
+	bool first = true;
 	int nout = -1;
-	for (auto &p : m->parts) {
+	for (size_t i = 0; i < m->parts.size(); i++) {
+		const Part &p = m->parts[i];
+		if (ns && std::all_of(ns + p.s0, ns + p.s0 + p.ns, [](size_t c) { return c == 0; })) continue;
 		const size_t off = (size_t)p.s0 * stride * sample_bytes;
 		const void *a = (const char *)x + off, *b = x2 ? (const char *)x2 + off : nullptr;
-		const int r = flag == ACB_FLAG_REAL_INPUT ? acb_submit_real_host(p.ctx, (const float *)a, stride, nsamples)
-		            : b ? acb_submit_cs16_planar_host(p.ctx, (const int16_t *)a, (const int16_t *)b, stride, nsamples)
-		                : acb_submit_cs16_host(p.ctx, (const int16_t *)a, stride, nsamples);
+		int r;
+		if (ns) {
+			size_t *o = &got[p.s0];
+			const size_t *c = ns + p.s0;
+			r = flag == ACB_FLAG_REAL_INPUT ? acb_submit_real_host_ragged(p.ctx, (const float *)a, stride, c, o)
+			    : b ? acb_submit_cs16_planar_host_ragged(p.ctx, (const int16_t *)a, (const int16_t *)b, stride, c, o)
+			        : acb_submit_cs16_host_ragged(p.ctx, (const int16_t *)a, stride, c, o);
+		} else {
+			r = flag == ACB_FLAG_REAL_INPUT ? acb_submit_real_host(p.ctx, (const float *)a, stride, nsamples)
+			    : b ? acb_submit_cs16_planar_host(p.ctx, (const int16_t *)a, (const int16_t *)b, stride, nsamples)
+			        : acb_submit_cs16_host(p.ctx, (const int16_t *)a, stride, nsamples);
+			std::fill(got.begin() + p.s0, got.begin() + p.s0 + p.ns, r < 0 ? 0 : (size_t)r);
+		}
 		if (r < 0) return r;
-		if (nout >= 0 && r != nout) return fail(ACB_ERR_CUDA, "parts of a multi-context produced %d and %d envelope samples", nout, r);
-		nout = r;
+		if (!first && (ns ? !std::equal(got.begin() + p.s0, got.begin() + p.s0 + p.ns, rows.begin() + p.s0) && m->mode == ACB_MULTI_SPLIT_CHANNELS
+		                  : r != nout))
+			return fail(ACB_ERR_CUDA, "parts of a multi-context produced different envelope samples");
+		std::copy(got.begin() + p.s0, got.begin() + p.s0 + p.ns, rows.begin() + p.s0);
+		nout = std::max(nout, r);
+		ran[i] = r > 0;
+		first = false;
 	}
-	if (nout > 0) {
-		const auto g = acb::stream_groups(m->group_unit, m->group_period, m->cfg.K, m->pos, (size_t)nout);
-		m->gstarts.insert(m->gstarts.end(), g.begin(), g.end());
-		m->gcount.push_back(g.size());
-		m->pos += (unsigned long long)nout;
-	}
+	if (nout > 0) record_submit(m, rows, std::move(ran));
+	if (nout_s) std::copy(rows.begin(), rows.end(), nout_s);
 	return nout;
 }
 
@@ -227,6 +286,27 @@ extern "C" int acb_multi_submit_cs16_planar_host(acb_multi_t *m, const int16_t *
 	return submit_streaming(m, ACB_FLAG_CS16_INPUT, xi, xq, sizeof(int16_t), stream_stride_samples, nsamples);
 }
 
+extern "C" int acb_multi_submit_real_host_ragged(acb_multi_t *m, const float *x, size_t stream_stride_samples, const size_t *nsamples,
+                                                 size_t *nout)
+{
+	if (!m || !x || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	return submit_streaming(m, ACB_FLAG_REAL_INPUT, x, nullptr, sizeof(float), stream_stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_multi_submit_cs16_host_ragged(acb_multi_t *m, const int16_t *iq, size_t stream_stride_samples, const size_t *nsamples,
+                                                 size_t *nout)
+{
+	if (!m || !iq || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	return submit_streaming(m, ACB_FLAG_CS16_INPUT, iq, nullptr, 2 * sizeof(int16_t), stream_stride_samples, 0, nsamples, nout);
+}
+
+extern "C" int acb_multi_submit_cs16_planar_host_ragged(acb_multi_t *m, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples,
+                                                        const size_t *nsamples, size_t *nout)
+{
+	if (!m || !xi || !xq || !nsamples) return fail(ACB_ERR_ARG, "null argument");
+	return submit_streaming(m, ACB_FLAG_CS16_INPUT, xi, xq, sizeof(int16_t), stream_stride_samples, 0, nsamples, nout);
+}
+
 /* pull what every part has queued, translate to global indices, merge in emission order */
 static int gather(acb_multi *m)
 {
@@ -239,26 +319,27 @@ static int gather(acb_multi *m)
 				buf[i].chn += p.c0;
 				m->scratch.push_back(buf[i]);
 			}
-	if (m->streaming) {
-		/* (group, stream, channel, time), as one context's consumer orders a streaming submit (context.cu) */
-		const auto &gs = m->gstarts;
-		auto group = [&gs](const acb_msg_t &x) { return std::upper_bound(gs.begin(), gs.end(), x.pos) - gs.begin(); };
-		std::stable_sort(m->scratch.begin(), m->scratch.end(), [&group](const acb_msg_t &a, const acb_msg_t &b) {
-			const auto ga = group(a), gb = group(b);
-			if (ga != gb) return ga < gb;
-			if (a.stream != b.stream) return a.stream < b.stream;
-			if (a.chn != b.chn) return a.chn < b.chn;
-			return a.pos < b.pos;
-		});
-	} else {
-		std::stable_sort(m->scratch.begin(), m->scratch.end(), [](const acb_msg_t &a, const acb_msg_t &b) {
-			if (a.block != b.block) return a.block < b.block;
-			if (a.stream != b.stream) return a.stream < b.stream;
-			if (a.chn != b.chn) return a.chn < b.chn;
-			return a.pos < b.pos;
-		});
+	/* (submit, group number counted from the stream's start, stream, channel, time), as one context's consumer orders
+	 * its submits (context.cu) */
+	struct Key { size_t sub; unsigned long long grp; };
+	std::vector<Key> key(m->scratch.size());
+	for (size_t i = 0; i < key.size(); i++) {
+		const acb_msg_t &x = m->scratch[i];
+		size_t sub = 0;
+		while (sub < m->subs.size() && m->subs[sub].end[x.stream] <= x.pos) sub++;
+		key[i] = Key{ sub, acb::group_number(!m->streaming, m->group_unit, m->group_period, m->cfg.K, x.pos) };
 	}
-	for (auto &x : m->scratch) m->outq.push_back(x);
+	std::vector<size_t> order(key.size());
+	for (size_t i = 0; i < order.size(); i++) order[i] = i;
+	std::stable_sort(order.begin(), order.end(), [m, &key](size_t ia, size_t ib) {
+		const acb_msg_t &a = m->scratch[ia], &b = m->scratch[ib];
+		if (key[ia].sub != key[ib].sub) return key[ia].sub < key[ib].sub;
+		if (key[ia].grp != key[ib].grp) return key[ia].grp < key[ib].grp;
+		if (a.stream != b.stream) return a.stream < b.stream;
+		if (a.chn != b.chn) return a.chn < b.chn;
+		return a.pos < b.pos;
+	});
+	for (size_t i : order) m->outq.push_back(m->scratch[i]);
 	return (int)m->outq.size();
 }
 
@@ -266,12 +347,13 @@ extern "C" int acb_multi_collect(acb_multi_t *m)
 {
 	if (!m) return ACB_ERR_ARG;
 	int err = 0;
-	for (auto &p : m->parts) { const int r = acb_collect(p.ctx); if (r < 0 && !err) err = r; }
-	const int n = gather(m);
-	if (!m->gcount.empty()) {                /* the oldest submit is merged: its groups are done */
-		m->gstarts.erase(m->gstarts.begin(), m->gstarts.begin() + m->gcount.front());
-		m->gcount.pop_front();
+	for (size_t i = 0; i < m->parts.size(); i++) {      /* the parts that ran the oldest submit */
+		if (!m->subs.empty() && !m->subs.front().part[i]) continue;
+		const int r = acb_collect(m->parts[i].ctx);
+		if (r < 0 && !err) err = r;
 	}
+	const int n = gather(m);
+	if (!m->subs.empty()) m->subs.pop_front();          /* the oldest submit is merged */
 	return err ? err : n;
 }
 
@@ -281,9 +363,24 @@ extern "C" int acb_multi_sync(acb_multi_t *m)
 	int err = 0;
 	for (auto &p : m->parts) { const int r = acb_sync(p.ctx); if (r < 0 && !err) err = r; }
 	const int n = gather(m);
-	m->gstarts.clear();
-	m->gcount.clear();
+	m->subs.clear();
 	return err ? err : n;
+}
+
+/* The submits in flight are collected first (as acb_multi_sync does): a message's submit is known from its stream's
+ * positions, which restart here. */
+extern "C" int acb_multi_reset_stream(acb_multi_t *m, int stream)
+{
+	if (!m) return fail(ACB_ERR_ARG, "null argument");
+	if (stream < 0 || stream >= m->cfg.nstreams) return fail(ACB_ERR_ARG, "stream %d out of range", stream);
+	const int r = acb_multi_sync(m);
+	if (r < 0) return r;
+	for (auto &p : m->parts) {
+		if (stream < p.s0 || stream >= p.s0 + p.ns) continue;
+		if (int e = acb_reset_stream(p.ctx, stream - p.s0)) return e;
+	}
+	m->spos[stream] = 0;
+	return ACB_OK;
 }
 
 extern "C" int acb_multi_drain(acb_multi_t *m, acb_msg_t *out, int max)

@@ -36,6 +36,12 @@ def stream_range(total_streams: int, world: int, rank: int) -> range:
     return split_range(total_streams, world, rank)
 
 
+def rank_counts(counts, total_streams: int, world: int, rank: int):
+    """The per-stream counts of a ragged submit that this rank's streams (stream_range) take."""
+    r = stream_range(total_streams, world, rank)
+    return counts[r.start:r.stop]
+
+
 def channel_range(nch: int, world: int, rank: int) -> range:
     return split_range(nch, world, rank)
 
@@ -108,6 +114,21 @@ def stream_groups(unit: int, period: int, K: int, pos: int, nout: int) -> list:
                 g.append(b)
             t += 1
     return g
+
+
+def group_number(unit: int | None, period: int, K: int, pos: int) -> int:
+    """The number, counted from the stream's start, of the emission group holding envelope sample `pos` (the context's
+    rule for streams at different positions, acb_set_emission_groups): unit None is u8 IQ, a group per 1024-row block;
+    GROUP_OUTPUTS one per `period` outputs; GROUP_INPUT the transfers' first outputs t*period // K (t >= 1) in (0, pos];
+    GROUP_SUBMIT numbers none (the submit is the group).  Within a submit frames leave in (group_number, stream, channel,
+    time) order."""
+    if unit is None:
+        return pos // 1024
+    if unit == GROUP_OUTPUTS:
+        return pos // period
+    if unit == GROUP_INPUT:
+        return ((pos + 1) * K - 1) // period if period >= K else pos
+    return 0
 
 
 def group_of(starts: Sequence[int], pos: int) -> int:

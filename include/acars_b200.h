@@ -306,6 +306,14 @@ int acb_set_wf(acb_ctx_t *ctx, int stream, const float *wf, int nch);
  * are abandoned with their frames.  The streaming submits' carried remainder (the samples that did not fill a row)
  * and the taps > K history are discarded: row 0 after a reset starts with the next sample submitted. */
 int acb_reset(acb_ctx_t *ctx);
+/* initMsk + initAcars for one stream's channels only, for a receiver that was retuned, stalled or reconnected: its
+ * carried remainder and taps > K history are discarded, its position returns to 0 (the next submit starts it at row 0,
+ * as after acb_reset) and, with ACB_FLAG_DECODE_STATS, its counts restart from nothing: they cover the submits made after
+ * the reset only.  Submits already made are still delivered (their messages, not their counts).  The other streams are
+ * not touched and nothing waits on the device: the reset is queued behind the work already submitted.  To retune one receiver, call
+ * acb_set_plan* (or acb_set_wf) for its stream, then acb_reset_stream; the planners wait for the submits in flight
+ * before they replace the stream's tables. */
+int acb_reset_stream(acb_ctx_t *ctx, int stream);
 
 /* ---- processing ---- */
 
@@ -353,6 +361,36 @@ int acb_submit_real_device(acb_ctx_t *ctx, const float *x_dev, size_t stream_str
 int acb_submit_cs16_device(acb_ctx_t *ctx, const int16_t *iq_dev, size_t stream_stride_samples, size_t nsamples);
 int acb_submit_cs16_planar_device(acb_ctx_t *ctx, const int16_t *xi_dev, const int16_t *xq_dev,
                                   size_t stream_stride_samples, size_t nsamples);
+/* Independent receivers: the ragged form of every submit above takes a count per stream — nblk[s] blocks, or
+ * nsamples[s] samples — so that each stream advances at its own pace.  Arguments are otherwise the lockstep calls':
+ *   - A count of 0 is allowed: the stream does not advance.  A call whose counts are all 0 is refused (ACB_ERR_ARG).
+ *   - The lockstep refusals hold per stream (wrong kind, a count above the cap, alignment), and with several streams the
+ *     stride must hold the largest count.  A refused call reads nothing and leaves every carry unchanged.
+ *   - The streaming calls write each stream's new envelope rows to nout[s] (nout may be NULL) and return the largest of
+ *     them, or a negative error.
+ *   - Stream s's envelope rows, messages, chain states and decode statistics are bit-identical to those of a one-stream
+ *     context of the same configuration fed only stream s's samples with the same cuts, for every input kind and
+ *     channelizer form.  With every count equal a ragged call is the lockstep call, bits and emission order alike, and a
+ *     context may mix lockstep and ragged calls, host and device.
+ *   - Input: the host calls read each stream's own count, except that every stream but the last is read up to the
+ *     largest count (within its stride).  acb_submit_device_ragged's channelizer reads every stream, the last one
+ *     included, for the largest nblk: each stream's region must be readable that far (the rows past its own count are
+ *     computed and never used).  The streaming device calls read each stream's own count.
+ *   - acb_read_dm keeps its layout with nsamp = the largest count of rows; stream s's rows at or beyond its own count are
+ *     unspecified.
+ *   - Lifetime and ordering: those of the lockstep calls. */
+int acb_submit_host_ragged(acb_ctx_t *ctx, const uint8_t *iq, size_t stream_stride, const int *nblk);
+int acb_submit_device_ragged(acb_ctx_t *ctx, const uint8_t *iq_dev, size_t stream_stride, const int *nblk);
+int acb_submit_real_host_ragged(acb_ctx_t *ctx, const float *x, size_t stream_stride_samples, const size_t *nsamples, size_t *nout);
+int acb_submit_cs16_host_ragged(acb_ctx_t *ctx, const int16_t *iq, size_t stream_stride_samples, const size_t *nsamples, size_t *nout);
+int acb_submit_cs16_planar_host_ragged(acb_ctx_t *ctx, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples,
+                                       const size_t *nsamples, size_t *nout);
+int acb_submit_real_device_ragged(acb_ctx_t *ctx, const float *x_dev, size_t stream_stride_samples, const size_t *nsamples,
+                                  size_t *nout);
+int acb_submit_cs16_device_ragged(acb_ctx_t *ctx, const int16_t *iq_dev, size_t stream_stride_samples, const size_t *nsamples,
+                                  size_t *nout);
+int acb_submit_cs16_planar_device_ragged(acb_ctx_t *ctx, const int16_t *xi_dev, const int16_t *xq_dev, size_t stream_stride_samples,
+                                         const size_t *nsamples, size_t *nout);
 /* Emission order of the streaming front-ends (SURVEY H5).  The reference runs demodMSK channel by channel on
  * whatever a transfer (air.c:336) or a full dm_buffer (soapy.c:247: 1024 outputs; sdrplay.c:229: 512) delivered, so
  * its messages leave in (group, channel, time) order.  A submit may carry many such groups; tell the context how
@@ -360,7 +398,12 @@ int acb_submit_cs16_planar_device(acb_ctx_t *ctx, const int16_t *xi_dev, const i
  *   ACB_GROUP_SUBMIT   one group per submit call (default);
  *   ACB_GROUP_OUTPUTS  a group every `period` envelope samples, counted from the start of the stream;
  *   ACB_GROUP_INPUT    a group per transfer of `period` input samples, counted from the start of the stream.
- * (u8 IQ contexts always group per 1024-sample block, rtl.c:357-360.) */
+ * (u8 IQ contexts always group per 1024-sample block, rtl.c:357-360.)
+ * Every stream counts its groups from its own start (acb_create, acb_reset, acb_reset_stream).  Within a submit the frames
+ * leave in (group number, stream, channel, time) order, the group number being the stream's 1024-row block (u8), the
+ * `period`-output group or the transfer (the first output each transfer completes) it lies in; with ACB_GROUP_SUBMIT
+ * the submit is one group.  When every stream is at the same position, as with lockstep calls only, this is the order
+ * above. */
 enum { ACB_GROUP_SUBMIT = 0, ACB_GROUP_OUTPUTS = 1, ACB_GROUP_INPUT = 2 };
 int acb_set_emission_groups(acb_ctx_t *ctx, int unit, uint64_t period);
 /* Replaces demodMSK's input side (msk.c:67; soundfile.c:71-77): 12.5 kS/s envelope samples,
@@ -506,6 +549,18 @@ int  acb_multi_set_plan_cs16(acb_multi_t *m, int stream, const unsigned *freqs_h
 int  acb_multi_submit_real_host(acb_multi_t *m, const float *x, size_t stream_stride_samples, size_t nsamples);
 int  acb_multi_submit_cs16_host(acb_multi_t *m, const int16_t *iq, size_t stream_stride_samples, size_t nsamples);
 int  acb_multi_submit_cs16_planar_host(acb_multi_t *m, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples, size_t nsamples);
+/* The ragged forms (see acb_submit_host_ragged).  A stream split hands each part its streams' counts; a part whose counts
+ * are all 0 sits the submit out.  A channel split hands every part all the counts, and the parts must agree on every
+ * nout[s] (ACB_ERR_CUDA otherwise).  The counts are checked before any part reads anything. */
+int  acb_multi_submit_host_ragged(acb_multi_t *m, const uint8_t *iq, size_t stream_stride, const int *nblk);
+int  acb_multi_submit_real_host_ragged(acb_multi_t *m, const float *x, size_t stream_stride_samples, const size_t *nsamples, size_t *nout);
+int  acb_multi_submit_cs16_host_ragged(acb_multi_t *m, const int16_t *iq, size_t stream_stride_samples, const size_t *nsamples,
+                                       size_t *nout);
+int  acb_multi_submit_cs16_planar_host_ragged(acb_multi_t *m, const int16_t *xi, const int16_t *xq, size_t stream_stride_samples,
+                                              const size_t *nsamples, size_t *nout);
+/* acb_reset_stream on the parts serving `stream`.  The submits in flight are collected first, as acb_multi_sync collects
+ * them (their messages wait in the output queue): the merge tells a message's submit by its stream's position. */
+int  acb_multi_reset_stream(acb_multi_t *m, int stream);
 int  acb_multi_set_emission_groups(acb_multi_t *m, int unit, uint64_t period);
 int  acb_multi_collect(acb_multi_t *m);
 int  acb_multi_sync(acb_multi_t *m);

@@ -105,4 +105,29 @@ for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
                 planes = dev.permute(2, 0, 1).contiguous()
                 assert ctx.submit_tensor(planes[0, :, :n], planes[1, :, :n]) == 3
         ctx.sync()
+# ragged submits: u8 device input with unequal nblk (the channelizer reads every stream, the last included, for the
+# largest nblk: the buffer ends there) and the taps > K history gather; the streaming kinds' ragged device submits
+# (k_append4_ragged behind unequal carries, k_move_tail), a stream at count 0 among them
+with api.Context(K, 3, 3, 2, flags=1, taps=2 * K + 3) as ctx:
+    for s in range(3):
+        ctx.set_plan(s, fd[:3])
+    bb = 1024 * K * 2
+    dev = torch.randint(0, 256, (3, 2 * bb), dtype=torch.uint8, device="cuda")
+    for counts in ([2, 0, 1], [1, 2, 0], [0, 1, 2]):
+        ctx.submit_device(dev.data_ptr(), 0, 2 * bb, counts=counts)
+    ctx.sync()
+for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
+    with api.Context(Kd, 3, 3, 1, flags=fl, taps=2 * Kd + 3) as ctx:
+        for s in range(3):
+            ctx.set_plan_air(s, fda) if kind == "real" else ctx.set_plan_cs16(s, fd[:3], 0)
+        n = 3 * Kd + 7
+        dev = (torch.randn((3, n), device="cuda") * 100 if kind == "real"
+               else torch.randint(-3000, 3000, (3, n, 2), dtype=torch.int16, device="cuda"))
+        for counts in ([77, 0, n], [n, 5, 0], [0, n, Kd + 1]):
+            if kind == "planar":
+                planes = dev.permute(2, 0, 1).contiguous()
+                ctx.submit_tensor(planes[0], planes[1], counts=counts)
+            else:
+                ctx.submit_tensor(dev, counts=counts)
+        ctx.sync()
 print("sanitize run ok", n1, n3, n4, n5)
