@@ -99,13 +99,33 @@ struct Hist {
 	int hpad;
 	unsigned long long pos0;
 };
-int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
-                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, CUstream_st *stream);
-int launch_channelize_generic(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
-                              int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp, CUstream_st *stream);
-int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
-                                  int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
-                                  const Hist &h, CUstream_st *stream);
+/* K1, the channelizer: the form a context runs (chan_form, kernels.cu, holds the table of which form applies when) */
+enum ChanForm { CHAN_EXACT, CHAN_GENERIC, CHAN_DFT, CHAN_RDFT, CHAN_OVL_FAST, CHAN_OVL_RDFT, CHAN_WB, CHAN_WB_REAL };
+ChanForm chan_form(int in_kind, int K, int taps, int flags);
+/* One channelizer launch: `form` over `nstreams` streams of input `in` (stream s at in + s*stride bytes) into
+ * dm[stream][nsamp][nch], with the context's tables (each stream's own rows of them, see chan_stream).  The streaming
+ * kinds' history sits right in front of the rows (hist.base = in - hpad samples, hist.stride = stride). */
+struct ChanLaunch {
+	ChanForm form;
+	int in_kind;                 /* IN_KIND_* */
+	const uint8_t *in;
+	size_t stride;
+	Hist hist;
+	const float *wf, *p, *tw;
+	const unsigned *twmeta;
+	const float *wbE;
+	const int *wbmeta;
+	float *dm;
+	int K, taps_pad, nch, nstreams;
+	size_t nsamp;                /* rows per stream of dm */
+	bool fold8;
+};
+/* Rows [0, nrows) of every stream of L: EXACT through the block kernel over whole 1024-row blocks and the generic kernel
+ * over the rest, GENERIC through the generic kernel; the fast forms take every row (nrows == nsamp).  Adds the kernels it
+ * launches to `launched`; returns a cudaError_t. */
+int launch_chan(const ChanLaunch &L, size_t nrows, CUstream_st *stream, int &launched);
+/* stream s of L alone, its window's terms before the stream start omitted from position pos0 */
+ChanLaunch chan_stream(const ChanLaunch &L, int s, unsigned long long pos0);
 /* nrows != NULL (device array): the ragged form, stream s demodulates its first nrows[s] <= nsamp rows (lanes 1, 2, 4 or 8
  * only: anything else returns cudaErrorInvalidValue) */
 int launch_demod(ChainState *st, const float *dm, int nsamp, int nch, int nstreams,
@@ -117,22 +137,6 @@ int launch_demod_stats(ChainState *st, const float *dm, int nsamp, int nch, int 
                        RawFrame *ring, RingCtl *ctl, unsigned cap, int lanes_per_channel, unsigned *counts, CUstream_st *stream,
                        const int *nrows = nullptr);
 int demod_pick_lanes(long long nchains, int sm_count);
-bool channelize_dft_supports(int K);
-int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                          int K, int nch, int nstreams, int nblk, size_t nsamp, bool fold8, CUstream_st *stream);
-int launch_channelize_dft_cs16(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                               int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
-int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
-                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
-int launch_channelize_wb(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *E,
-                         const int *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
-bool channelize_rdft_supports(int K);
-int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                           int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
-int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
-                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
-int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
-                              float *dm, int K, int nch, int nstreams, size_t nsamp, CUstream_st *stream);
 int launch_block_fec(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);
 /* the same repair, and each frame's FEC_WHY_* in RawFrame::pad1[0] */
 int launch_block_fec_stats(RawFrame *ring, const RingCtl *ctl, unsigned cap, CUstream_st *stream);

@@ -72,24 +72,6 @@ struct EvTriple { cudaEvent_t a, b, b2, c; bool chan; };   /* a..b = K1 on s_com
  * behind that of N+1 and both kernels run back to back on their streams. */
 constexpr int NPIPE = 3;
 
-/* K1, the channelizer: the form a context runs, chosen once by chan_form() and tried in this order
- *
- *   input       condition                                                      form
- *   u8 / CS16   ACB_FLAG_FAST_CHANNELIZER, taps == K, K in {160, 192}          CHAN_DFT       k_channelize_dft(1)
- *               ACB_FLAG_FAST_FILTER, taps > K, K in {160, 192}                CHAN_OVL_FAST  k_channelize_ovl_fast
- *               ACB_FLAG_FAST_WIDEBAND, taps >= K, K % 8 == 0                  CHAN_WB        k_channelize_wb
- *               K % 8 != 0 (u8), K % 4 != 0 (CS16)                             CHAN_GENERIC   k_channelize_generic(_ovl)
- *               otherwise                                                      CHAN_EXACT     k_channelize_iq4
- *   real        ACB_FLAG_FAST_CHANNELIZER, taps == K, channelize_rdft_supports  CHAN_RDFT      k_channelize_rdft
- *               ACB_FLAG_FAST_FILTER_REAL, taps > K, channelize_rdft_supports  CHAN_OVL_RDFT  k_channelize_ovl_rdft
- *               ACB_FLAG_FAST_WIDEBAND_REAL, taps >= K, K % 8 == 0             CHAN_WB_REAL   k_channelize_wb_real
- *               K % 4 != 0                                                     CHAN_GENERIC   k_channelize_generic(_ovl)
- *               otherwise                                                      CHAN_EXACT     k_channelize_real4
- *
- * A fast form (all but EXACT and GENERIC) runs only while every stream is planned on the 12.5 kHz raster (fast_ok); a
- * submit runs EXACT otherwise. */
-enum ChanForm { CHAN_EXACT, CHAN_GENERIC, CHAN_DFT, CHAN_RDFT, CHAN_OVL_FAST, CHAN_OVL_RDFT, CHAN_WB, CHAN_WB_REAL };
-
 /* Emission-order groups of one submit (input blocks / chunks).  Even submits (every stream at the same position):
  * `starts` holds the groups every stream shares and `off` is empty.  Otherwise stream s's groups are
  * starts[off[s] .. off[s+1]), and base[s] is the number, counted from the stream's own start, of its first one: frames
@@ -298,22 +280,6 @@ static int reset_states(acb_ctx *c)
 	return ACB_OK;
 }
 
-/* the table at ChanForm */
-static ChanForm chan_form(const acb_config_t *cfg, int in_kind, int taps)
-{
-	const int K = cfg->K, f = cfg->flags;
-	if (in_kind == IN_KIND_F32REAL) {
-		if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_rdft_supports(K)) return CHAN_RDFT;
-		if ((f & ACB_FLAG_FAST_FILTER_REAL) && taps > K && channelize_rdft_supports(K)) return CHAN_OVL_RDFT;
-		if ((f & ACB_FLAG_FAST_WIDEBAND_REAL) && taps >= K && K % 8 == 0) return CHAN_WB_REAL;
-		return K % 4 ? CHAN_GENERIC : CHAN_EXACT;
-	}
-	if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_dft_supports(K)) return CHAN_DFT;
-	if ((f & ACB_FLAG_FAST_FILTER) && taps > K && channelize_dft_supports(K)) return CHAN_OVL_FAST;
-	if ((f & ACB_FLAG_FAST_WIDEBAND) && taps >= K && K % 8 == 0) return CHAN_WB;
-	return K % (in_kind == IN_KIND_U8IQ ? 8 : 4) ? CHAN_GENERIC : CHAN_EXACT;
-}
-
 extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 {
 	if (!cfg || !out) return fail(ACB_ERR_ARG, "null argument");
@@ -341,7 +307,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->in_kind = (cfg->flags & ACB_FLAG_REAL_INPUT) ? IN_KIND_F32REAL : (cfg->flags & ACB_FLAG_CS16_INPUT) ? IN_KIND_CS16IQ : IN_KIND_U8IQ;
 	c->real_input = c->in_kind != IN_KIND_U8IQ;
 	c->taps = cfg->taps ? cfg->taps : cfg->K;
-	c->form = chan_form(cfg, c->in_kind, c->taps);
+	c->form = chan_form(c->in_kind, cfg->K, c->taps, cfg->flags);
 	{
 		const int per_unit = c->real_input ? 4 : 8;          /* taps per 16 bytes of input (4-byte vs 2-byte taps) */
 		c->hpad = 0;
@@ -1058,115 +1024,41 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		bool fast = c->form != CHAN_EXACT && c->form != CHAN_GENERIC;
 		for (int s = 0; fast && s < c->cfg.nstreams; s++) fast = c->fast_ok[s] != 0;
 		const ChanForm form = fast || c->form == CHAN_GENERIC ? c->form : CHAN_EXACT;
-		/* EXACT: whole 1024-row blocks through the block kernel, the remaining rows (submits of 4-byte samples may carry any
-		 * count) through the generic one; GENERIC (unaligned K): every row through the generic one */
-		const int blocks = form == CHAN_GENERIC ? 0 : nsamp / OUTBLK;
-		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
-		 * for the streaming kinds (submit4) */
 		/* streams at different positions (acb_reset_stream): the launch takes the furthest one, and the streams near their
 		 * start whose window reaches before it are redone below, one by one, at their own position */
 		const unsigned long long pos_max = *std::max_element(c->pos.begin(), c->pos.end());
 		const bool even_pos = std::all_of(c->pos.begin(), c->pos.end(), [&](unsigned long long p) { return p == pos_max; });
-		auto rows_of = [&](int s) { return h_rows ? (size_t)h_rows[s] : (size_t)nsamp; };
-		Hist hist{ nullptr, 0, c->hpad, pos_max };
-		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
-			hist.base = c->d_hist;
-			hist.stride = (size_t)c->hpad * 2;
-		} else if (c->hpad) {
-			hist.base = d_iq - (size_t)c->hpad * 4;
-			hist.stride = stride;
-		}
-		int r = 0;
-		switch (form) {
-		case CHAN_EXACT:
-		case CHAN_GENERIC:            /* blocks == 0 */
-			if (blocks)
-				r = launch_channelize(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, blocks,
-				                      (size_t)nsamp, hist, c->s_comp);
-			break;
-		case CHAN_DFT:
-			r = c->in_kind == IN_KIND_CS16IQ
-			        ? launch_channelize_dft_cs16(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp,
-			                                     c->s_comp)
-			        : launch_channelize_dft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, blocks, (size_t)nsamp,
-			                                c->fold8, c->s_comp);
-			break;
-		case CHAN_RDFT:
-			r = launch_channelize_rdft(d_iq, stride, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			break;
-		case CHAN_OVL_FAST:
-			r = launch_channelize_ovl_fast(c->in_kind, d_iq, stride, hist, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			break;
-		case CHAN_OVL_RDFT:
-			/* the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
-			r = launch_channelize_ovl_rdft(d_iq, stride, c->hpad, c->d_p, c->d_tw, c->d_twmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                               c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			break;
-		case CHAN_WB:
-			/* at taps > K the terms before the stream start are omitted in the kernel */
-			r = launch_channelize_wb(c->in_kind, d_iq, stride, hist, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                         c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			break;
-		case CHAN_WB_REAL:
-			/* at taps > K the history sits right in front of each stream's rows in d_real (submit4), zeros after create / reset */
-			r = launch_channelize_wb_real(d_iq, stride, c->hpad, c->d_p, c->d_wbE, c->d_wbmeta, dmbuf, c->cfg.K, c->cfg.nch,
-			                              c->cfg.nstreams, (size_t)nsamp, c->s_comp);
-			break;
-		}
-		if (fast || blocks) c->stats.kernel_launches++;          /* the fast kernel, or EXACT's block kernel */
-		if (!r && !even_pos && c->hpad && (form == CHAN_OVL_FAST || form == CHAN_WB)) {
-			/* these forms omit the terms before the stream start themselves, from hist.pos0: a stream whose window still
-			 * reaches there (within (hpad + K - 1) / K rows of its start) is redone alone at its own position */
-			const unsigned long long reach = ((unsigned long long)c->hpad + c->cfg.K - 1) / c->cfg.K;
-			const size_t wf_per = (size_t)c->ngrp * CH_GROUP * (c->cfg.K / 4) * 2;
-			const size_t nct = (size_t)(c->cfg.nch + WB_CTILE - 1) / WB_CTILE;
-			for (int s = 0; !r && s < c->cfg.nstreams; s++) {
-				if (c->pos[s] >= reach || rows_of(s) == 0) continue;
-				Hist h1{ (const uint8_t *)hist.base + (size_t)s * hist.stride, hist.stride, c->hpad, c->pos[s] };
-				const uint8_t *in1 = d_iq + (size_t)s * stride;
-				float *dm1 = dmbuf + (size_t)s * nsamp * c->cfg.nch;
-				r = form == CHAN_OVL_FAST
-				        ? launch_channelize_ovl_fast(c->in_kind, in1, stride, h1, c->d_p, c->d_tw + s * wf_per, c->d_twmeta + (size_t)s * c->ngrp,
-				                                     dm1, c->cfg.K, c->cfg.nch, 1, (size_t)nsamp, c->s_comp)
-				        : launch_channelize_wb(c->in_kind, in1, stride, h1, c->d_p, c->d_wbE, c->d_wbmeta + s * nct * WB_META, dm1, c->cfg.K,
-				                               c->cfg.nch, 1, (size_t)nsamp, c->s_comp);
-				c->stats.kernel_launches++;
+		/* taps > K: where each stream's history sits — the u8 history buffer, or right in front of the input in d_real
+		 * for the streaming kinds (submit4), zeros after create / reset */
+		const Hist hist = !c->hpad                         ? Hist{ nullptr, 0, 0, pos_max }
+		                  : c->in_kind == IN_KIND_U8IQ ? Hist{ c->d_hist, (size_t)c->hpad * 2, c->hpad, pos_max }
+		                                               : Hist{ d_iq - (size_t)c->hpad * 4, stride, c->hpad, pos_max };
+		ChanLaunch L{ form, c->in_kind, d_iq, stride, hist, c->d_wf, c->d_p, c->d_tw, c->d_twmeta, c->d_wbE, c->d_wbmeta,
+		              dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams, (size_t)nsamp, c->fold8 };
+		int launched = 0;
+		int r = launch_chan(L, (size_t)nsamp, c->s_comp, launched);
+		/* taps > K, streams near their start.  OVL_FAST and WB omit the window terms before the stream start themselves,
+		 * from hist.pos0: at different positions a stream within ceil(hpad / K) rows of its start is redone alone, every
+		 * row.  u8 EXACT's block kernel took the zero history bytes (-127.37 after conversion) as terms, and so did
+		 * GENERIC's launch at pos_max for the streams behind it: their first ceil(H / K) rows after their start go through
+		 * the generic kernel again, which omits those terms — all streams in one launch when they sit at the same position.
+		 * The other forms read history that converts to 0, which is the omitted terms exactly. */
+		const bool own = form == CHAN_OVL_FAST || form == CHAN_WB;
+		if (!r && c->hpad && (own || (c->in_kind == IN_KIND_U8IQ && (form == CHAN_EXACT || form == CHAN_GENERIC)))) {
+			const unsigned long long K = (unsigned long long)c->cfg.K, reach = ((own ? c->hpad : c->taps - c->cfg.K) + K - 1) / K;
+			L.form = own ? form : CHAN_GENERIC;
+			if (even_pos && form == CHAN_EXACT && pos_max < reach)
+				r = launch_chan(L, (size_t)std::min<unsigned long long>(reach - pos_max, (unsigned long long)nsamp), c->s_comp, launched);
+			for (int s = 0; !r && !even_pos && s < c->cfg.nstreams; s++) {
+				const size_t rows = h_rows ? (size_t)h_rows[s] : (size_t)nsamp;
+				if (c->pos[s] >= reach || rows == 0) continue;
+				r = launch_chan(chan_stream(L, s, c->pos[s]), own ? (size_t)nsamp : std::min<size_t>(reach - c->pos[s], rows), c->s_comp,
+				                launched);
 			}
 		}
+		c->stats.kernel_launches += launched;
 		if (fast) c->stats.fast_chan_launches++;
-		if (!r && !fast && nsamp > blocks * OUTBLK) {
-			const size_t row0 = (size_t)blocks * OUTBLK, nrows = (size_t)nsamp - row0;
-			r = c->hpad ? launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch,
-			                                            c->cfg.nstreams, row0, nrows, (size_t)nsamp, hist, c->s_comp)
-			            : launch_channelize_generic(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
-			                                        row0, nrows, (size_t)nsamp, c->s_comp);
-			c->stats.kernel_launches++;
-		}
 		if (c->hpad && c->in_kind == IN_KIND_U8IQ) {
-			/* u8 history: the block kernel read zero bytes (-127.37 after conversion) for the samples before the stream
-			 * start; the rows whose window reaches there — at most ceil(H/K) <= 16 rows of the first submit after
-			 * create / reset — are recomputed with those terms omitted (GENERIC and the fast forms omit them themselves) */
-			const unsigned long long H = (unsigned long long)(c->taps - c->cfg.K), K = (unsigned long long)c->cfg.K;
-			const unsigned long long lead = (H + K - 1) / K;
-			if (!r && form == CHAN_EXACT && even_pos && pos_max < lead) {
-				r = launch_channelize_generic_ovl(c->in_kind, d_iq, stride, c->d_wf, dmbuf, c->cfg.K, c->taps_pad, c->cfg.nch, c->cfg.nstreams,
-				                                  0, (size_t)std::min<unsigned long long>(lead - pos_max, (unsigned long long)nsamp), (size_t)nsamp,
-				                                  hist, c->s_comp);
-				c->stats.kernel_launches++;
-			}
-			/* streams at different positions: EXACT's block kernel and GENERIC's launch (at pos_max) took the zero history
-			 * bytes as terms; redo the rows of each stream that reach before its start, stream by stream, at its own position */
-			const bool redo = form == CHAN_EXACT || form == CHAN_GENERIC;
-			for (int s = 0; !r && redo && !even_pos && s < c->cfg.nstreams; s++) {
-				if (c->pos[s] >= lead || rows_of(s) == 0) continue;
-				const Hist h1{ c->d_hist + (size_t)s * hist.stride, hist.stride, c->hpad, c->pos[s] };
-				r = launch_channelize_generic_ovl(c->in_kind, d_iq + (size_t)s * stride, stride,
-				                                  c->d_wf + (size_t)s * c->ngrp * c->taps_pad * CH_GROUP * 2, dmbuf + (size_t)s * nsamp * c->cfg.nch,
-				                                  c->cfg.K, c->taps_pad, c->cfg.nch, 1, 0,
-				                                  std::min<size_t>(lead - c->pos[s], rows_of(s)), (size_t)nsamp, h1, c->s_comp);
-				c->stats.kernel_launches++;
-			}
 			/* the input's last hpad samples are the next submit's history; the copy follows K1 on the same stream, so
 			 * K1 of the next submit sees it and the input-lifetime event below covers it */
 			const size_t hb = (size_t)c->hpad * 2, len = (size_t)nblk * c->blk_bytes;

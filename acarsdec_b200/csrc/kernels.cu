@@ -28,6 +28,7 @@
 
 #include <algorithm>
 
+#include "../../include/acars_b200.h"
 #include "acb_internal.h"
 #include "frame_sm.h"
 #include "demod_core.h"
@@ -490,6 +491,14 @@ k_channelize_real4(const uint8_t *__restrict__ in, size_t stream_stride, const u
 	}
 }
 
+/* a kernel's launch attributes: up to `smem` bytes of dynamic shared memory, and the largest shared-memory carve-out */
+template <typename F>
+static cudaError_t smem_max_carveout(F *kern, int smem)
+{
+	const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	return e != cudaSuccess ? e : cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+}
+
 template <bool OVL>
 static int launch_channelize_real4(const void *in, size_t stream_stride, const void *wf, float *dm,
                                    int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
@@ -497,10 +506,7 @@ static int launch_channelize_real4(const void *in, size_t stream_stride, const v
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	const size_t smem = 2 * (size_t)(C2_ROWS * 5 * 16 + 20 * CH_GROUP * 8);
-	cudaError_t e = cudaFuncSetAttribute(k_channelize_real4<OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(k_channelize_real4<OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(k_channelize_real4<OVL>, (int)smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	k_channelize_real4<OVL><<<grid, R4_THREADS, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
 	                                                           reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
@@ -515,13 +521,10 @@ static int launch_channelize_real2(const void *in, size_t stream_stride, const v
 	if (nblk == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	const size_t smem = (size_t)C2::STAGES * C2::STAGE_BYTES;
-	cudaError_t e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-	if (e != cudaSuccess) return (int)e;
 	/* the largest shared-memory carve-out: the staging ring is this kernel's working set.  (Kernels that prefer
 	 * different splits do share an SM — the demod of submit i runs underneath the channelizer of submit i+1 whatever
 	 * the two ask for, see launch_channelize_iq4.) */
-	e = cudaFuncSetAttribute(k_channelize<OVL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(k_channelize<OVL>, (int)smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	k_channelize<OVL><<<grid, CH_TILE, smem, stream>>>(reinterpret_cast<const uint8_t *>(in), stream_stride,
 	                                                   reinterpret_cast<const uint8_t *>(wf), dm, K, taps, nch, ngrp, nsamp,
@@ -568,8 +571,8 @@ static int launch_channelize_k(int mode, const void *in, size_t stream_stride_by
 
 /* whole 1024-row blocks of any input kind; the caller sends remaining rows to the generic kernel.  h.hpad > 0 selects
  * the overlapping-window instantiations (taps = K + h.hpad) */
-int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
-                      int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
+static int launch_channelize(int mode, const void *in, size_t stream_stride_bytes, const float *wf, float *dm,
+                             int K, int taps, int nch, int nstreams, int nblk, size_t nsamp, const Hist &h, cudaStream_t stream)
 {
 	return h.hpad ? launch_channelize_k<true>(mode, in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream)
 	              : launch_channelize_k<false>(mode, in, stream_stride_bytes, wf, dm, K, taps, nch, nstreams, nblk, nsamp, h, stream);
@@ -897,10 +900,7 @@ static int launch_dft_t(const uint8_t *in, size_t stream_stride, const float2 *t
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	constexpr int smem = DftPlan<UNITS, WARPS, STAGES>::SMEM;
 	auto kern = k_channelize_dft<UNITS, WARPS, STAGES, MINB, FOLD8>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, tw, meta, dm, nch, ngrp, nsamp);
 	return (int)cudaGetLastError();
@@ -1132,10 +1132,7 @@ static int launch_dft1_t(const uint8_t *in, size_t stream_stride, const float2 *
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	constexpr int smem = Dft1Plan<KIND, UNITS, WARPS>::SMEM;
 	auto kern = k_channelize_dft1<KIND, UNITS, WARPS, MINB, PF>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, tw, meta, dm, nch, ngrp, nsamp);
 	return (int)cudaGetLastError();
@@ -1366,10 +1363,7 @@ static int launch_ovl_fast_t(const uint8_t *in, size_t stream_stride, const Hist
 	/* shared memory grows with the halo only: (32 + HR) rows per warp */
 	const int smem = WARPS * (DFT1_ROWS + HR) * (P::ROWBYTES + 16) + P::TW_BYTES + WARPS * 8;
 	auto kern = k_channelize_ovl_fast<KIND, UNITS, WARPS>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad, h.pos0,
 	                                         p, tw, meta, dm, nch, ngrp, nsamp);
@@ -1378,8 +1372,8 @@ static int launch_ovl_fast_t(const uint8_t *in, size_t stream_stride, const Hist
 
 /* u8 IQ or CS16 IQ, taps > K, K in {160, 192}, every channel on the 12.5 kHz raster; `nsamp` output rows per stream, any
  * count (CS16: the input buffer carries 32 rows of slack); `p` = taps_pad floats, fl(K*h) behind hpad - H zeros */
-int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
-                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_ovl_fast(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *tw,
+                                      const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
@@ -1605,10 +1599,7 @@ static int launch_wb_t(const uint8_t *in, size_t stream_stride, const Hist &h, c
 	const int smem = 4 * T * (K / 8) * 8 + (2 * K - 1) * 8;
 	const int nctile = (nch + WB_CTILE - 1) / WB_CTILE;
 	auto kern = k_channelize_wb<KIND, OVL, RB>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	const int rows_per_cta = wb_tiles_per_cta(nsamp, T, nstreams, nctile) * T;
 	dim3 grid((unsigned)((nsamp + rows_per_cta - 1) / rows_per_cta), nstreams, nctile);
 	kern<<<grid, WB_THREADS, smem, stream>>>(in, stream_stride, reinterpret_cast<const uint8_t *>(h.base), h.stride, h.hpad, h.pos0,
@@ -1618,8 +1609,8 @@ static int launch_wb_t(const uint8_t *in, size_t stream_stride, const Hist &h, c
 
 /* u8 IQ or CS16 IQ, K % 8 == 0, K <= ACB_MAXK, any nch, every channel on the 12.5 kHz raster; taps = K (h.hpad = 0) or
  * taps > K (`p` = taps_pad floats, fl(K*h) behind hpad - H zeros); `nsamp` output rows per stream, any count */
-int launch_channelize_wb(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *E,
-                         const int *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_wb(int mode, const void *in, size_t stream_stride, const Hist &h, const float *p, const float *E,
+                                const int *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	if ((K & 7) || K > 2048 || (mode != IN_U8IQ && mode != IN_CS16IQ)) return (int)cudaErrorInvalidValue;
@@ -1829,24 +1820,21 @@ static int launch_rdft_t(const uint8_t *in, size_t stream_stride, const float2 *
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	constexpr int smem = RdftPlan<K8, LPR, WARPS>::SMEM;
 	auto kern = k_channelize_rdft<K8, LPR, WARPS, MINB>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, tw, meta, dm, nch, ngrp, nsamp);
 	return (int)cudaGetLastError();
 }
 
 /* the Airspy rates: 2.5 MS/s (K = 200), 3 (240), 5 (400), 6 (480), 10 (800) */
-bool channelize_rdft_supports(int K) { return K == 200 || K == 240 || K == 400 || K == 480 || K == 800; }
+static bool channelize_rdft_supports(int K) { return K == 200 || K == 240 || K == 400 || K == 480 || K == 800; }
 /* lanes per row of k_channelize_rdft (the CPU restatement needs it: it fixes the order of the partial sums) */
 int channelize_rdft_lanes_per_row(int K) { return K >= 800 ? 8 : K >= 400 ? 4 : 2; }
 
 /* float32 real input (air.c), taps == K, every channel on the 12.5 kHz raster around Fc; `nsamp` output rows per stream,
  * any count (the input buffer carries 32 rows of slack).  stream_stride in bytes. */
-int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                           int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_rdft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
+                                  int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
@@ -2119,10 +2107,7 @@ static int launch_ovl_rdft_t(const uint8_t *in, size_t stream_stride, int hpad, 
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
 	const int smem = ovl_rdft_smem<K8, LPR, WARPS>(hpad);
 	auto kern = k_channelize_ovl_rdft<K8, LPR, WARPS, CW>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	dim3 grid(nblk, nstreams, ngrp);
 	kern<<<grid, 32 * WARPS, smem, stream>>>(in, stream_stride, hpad, p, tw, meta, dm, nch, ngrp, nsamp);
 	return (int)cudaGetLastError();
@@ -2131,8 +2116,8 @@ static int launch_ovl_rdft_t(const uint8_t *in, size_t stream_stride, int hpad, 
 /* float32 real input, taps > K (hpad > 0), K in the rdft's five rates, every channel on the 12.5 kHz raster; `in` = sample 0
  * of stream 0's submit with each stream's hpad-sample history right in front of it (d_real); `nsamp` output rows per
  * stream, any count; `p` = taps_pad floats, fl(K*h) behind hpad - H zeros */
-int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
-                               const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_ovl_rdft(const void *in, size_t stream_stride, int hpad, const float *p, const float *tw,
+                                      const unsigned *meta, float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	if (hpad <= 0 || hpad % 4) return (int)cudaErrorInvalidValue;           /* 16-byte copies; taps <= K has no history */
@@ -2347,10 +2332,7 @@ static int launch_wbr_t(const uint8_t *in, size_t stream_stride, int hpad, const
 	const int smem = 4 * T * K + 8 * K;
 	const int nctile = (nch + WB_CTILE - 1) / WB_CTILE;
 	auto kern = k_channelize_wb_real<LPR, OVL>;
-	cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	if (e != cudaSuccess) return (int)e;
-	e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-	if (e != cudaSuccess) return (int)e;
+	if (cudaError_t e = smem_max_carveout(kern, smem)) return (int)e;
 	const int rows_per_cta = wb_tiles_per_cta(nsamp, T, nstreams, nctile) * T;
 	dim3 grid((unsigned)((nsamp + rows_per_cta - 1) / rows_per_cta), nstreams, nctile);
 	kern<<<grid, WBR_THREADS, smem, stream>>>(in, stream_stride, hpad, p, E, meta, dm, K, nch, nctile, nsamp, T, rows_per_cta);
@@ -2360,8 +2342,8 @@ static int launch_wbr_t(const uint8_t *in, size_t stream_stride, int hpad, const
 /* float32 real input, K % 8 == 0, K <= ACB_MAXK, any nch, every channel on the 12.5 kHz raster; taps = K (hpad = 0) or
  * taps > K (`p` = taps_pad floats, fl(K*h) behind hpad - H zeros); `in` = sample 0 of stream 0's submit with each
  * stream's hpad-sample history right in front of it (d_real); `nsamp` output rows per stream, any count */
-int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
-                              float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, const float *p, const float *E, const int *meta,
+                                     float *dm, int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	if ((K & 7) || K > 2048 || hpad < 0) return (int)cudaErrorInvalidValue;
@@ -2374,12 +2356,12 @@ int launch_channelize_wb_real(const void *in, size_t stream_stride, int hpad, co
 #undef ACB_WBR_GO
 }
 
-bool channelize_dft_supports(int K) { return K == 160 || K == 192; }
+static bool channelize_dft_supports(int K) { return K == 160 || K == 192; }
 
 /* u8 IQ, K in {160, 192} (the reference's two rates), taps == K, every channel on the 12.5 kHz raster
  * around Fc (context.cu checks and builds tw/meta) */
-int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                          int K, int nch, int nstreams, int nblk, size_t nsamp, bool fold8, cudaStream_t stream)
+static int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
+                                 int K, int nch, int nstreams, int nblk, size_t nsamp, bool fold8, cudaStream_t stream)
 {
 	if (nblk == 0) return 0;
 	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
@@ -2411,8 +2393,8 @@ int launch_channelize_dft(const void *in, size_t stream_stride, const float *tw,
 
 /* CS16 IQ (soapy.c / sdrplay.c), same conditions as above; `nsamp` output rows per stream, any count: the last block may be
  * partial (the input buffer carries 32 rows of slack).  stream_stride in bytes. */
-int launch_channelize_dft_cs16(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
-                               int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_dft_cs16(const void *in, size_t stream_stride, const float *tw, const unsigned *meta, float *dm,
+                                      int K, int nch, int nstreams, size_t nsamp, cudaStream_t stream)
 {
 	if (nsamp == 0) return 0;
 	const uint8_t *i8 = reinterpret_cast<const uint8_t *>(in);
@@ -2605,8 +2587,8 @@ k_channelize_generic(const uint8_t *__restrict__ in, size_t stream_stride, const
 	dm[((size_t)s * nsamp + m) * nch + ch] = envelope(make_float2(dr, di));
 }
 
-int launch_channelize_generic(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
-                              int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp, cudaStream_t stream)
+static int launch_channelize_generic(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
+                                     int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp, cudaStream_t stream)
 {
 	if (nrows == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
@@ -2671,9 +2653,9 @@ k_channelize_generic_ovl(const uint8_t *__restrict__ in, size_t stream_stride, c
 	dm[((size_t)s * nsamp + m) * nch + ch] = envelope(make_float2(dr, di));
 }
 
-int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
-                                  int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
-                                  const Hist &h, cudaStream_t stream)
+static int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride, const void *wf, float *dm,
+                                         int K, int taps, int nch, int nstreams, size_t row0, size_t nrows, size_t nsamp,
+                                         const Hist &h, cudaStream_t stream)
 {
 	if (nrows == 0) return 0;
 	const int ngrp = (nch + CH_GROUP - 1) / CH_GROUP;
@@ -2687,6 +2669,91 @@ int launch_channelize_generic_ovl(int mode, const void *in, size_t stream_stride
 	else ACB_GEN_OVL(IN_U8IQ);
 #undef ACB_GEN_OVL
 	return (int)cudaGetLastError();
+}
+
+/* K1's forms, tried in this order (chan_form):
+ *
+ *   input       condition                                                      form
+ *   u8 / CS16   ACB_FLAG_FAST_CHANNELIZER, taps == K, K in {160, 192}          CHAN_DFT       k_channelize_dft(1)
+ *               ACB_FLAG_FAST_FILTER, taps > K, K in {160, 192}                CHAN_OVL_FAST  k_channelize_ovl_fast
+ *               ACB_FLAG_FAST_WIDEBAND, taps >= K, K % 8 == 0                  CHAN_WB        k_channelize_wb
+ *               K % 8 != 0 (u8), K % 4 != 0 (CS16)                             CHAN_GENERIC   k_channelize_generic(_ovl)
+ *               otherwise                                                      CHAN_EXACT     k_channelize_iq4
+ *   real        ACB_FLAG_FAST_CHANNELIZER, taps == K, channelize_rdft_supports  CHAN_RDFT      k_channelize_rdft
+ *               ACB_FLAG_FAST_FILTER_REAL, taps > K, channelize_rdft_supports  CHAN_OVL_RDFT  k_channelize_ovl_rdft
+ *               ACB_FLAG_FAST_WIDEBAND_REAL, taps >= K, K % 8 == 0             CHAN_WB_REAL   k_channelize_wb_real
+ *               K % 4 != 0                                                     CHAN_GENERIC   k_channelize_generic(_ovl)
+ *               otherwise                                                      CHAN_EXACT     k_channelize_real4
+ *
+ * A fast form (all but EXACT and GENERIC) runs only while every stream is planned on the 12.5 kHz raster; a submit runs
+ * EXACT otherwise (context.cu). */
+ChanForm chan_form(int in_kind, int K, int taps, int f)
+{
+	if (in_kind == IN_KIND_F32REAL) {
+		if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_rdft_supports(K)) return CHAN_RDFT;
+		if ((f & ACB_FLAG_FAST_FILTER_REAL) && taps > K && channelize_rdft_supports(K)) return CHAN_OVL_RDFT;
+		if ((f & ACB_FLAG_FAST_WIDEBAND_REAL) && taps >= K && K % 8 == 0) return CHAN_WB_REAL;
+		return K % 4 ? CHAN_GENERIC : CHAN_EXACT;
+	}
+	if ((f & ACB_FLAG_FAST_CHANNELIZER) && taps == K && channelize_dft_supports(K)) return CHAN_DFT;
+	if ((f & ACB_FLAG_FAST_FILTER) && taps > K && channelize_dft_supports(K)) return CHAN_OVL_FAST;
+	if ((f & ACB_FLAG_FAST_WIDEBAND) && taps >= K && K % 8 == 0) return CHAN_WB;
+	return K % (in_kind == IN_KIND_U8IQ ? 8 : 4) ? CHAN_GENERIC : CHAN_EXACT;
+}
+
+int launch_chan(const ChanLaunch &L, size_t nrows, cudaStream_t stream, int &launched)
+{
+	const int K = L.K, nch = L.nch, ns = L.nstreams;
+	const size_t nsamp = L.nsamp;
+	if (L.form != CHAN_EXACT && L.form != CHAN_GENERIC) {
+		if (nrows != nsamp) return (int)cudaErrorInvalidValue;
+		launched++;
+	}
+	switch (L.form) {
+	case CHAN_DFT:
+		return L.in_kind == IN_KIND_CS16IQ
+		           ? launch_channelize_dft_cs16(L.in, L.stride, L.tw, L.twmeta, L.dm, K, nch, ns, nsamp, stream)
+		           : launch_channelize_dft(L.in, L.stride, L.tw, L.twmeta, L.dm, K, nch, ns, (int)(nsamp / OUTBLK), nsamp, L.fold8, stream);
+	case CHAN_RDFT: return launch_channelize_rdft(L.in, L.stride, L.tw, L.twmeta, L.dm, K, nch, ns, nsamp, stream);
+	case CHAN_OVL_FAST:
+		return launch_channelize_ovl_fast(L.in_kind, L.in, L.stride, L.hist, L.p, L.tw, L.twmeta, L.dm, K, nch, ns, nsamp, stream);
+	case CHAN_OVL_RDFT:
+		return launch_channelize_ovl_rdft(L.in, L.stride, L.hist.hpad, L.p, L.tw, L.twmeta, L.dm, K, nch, ns, nsamp, stream);
+	case CHAN_WB: return launch_channelize_wb(L.in_kind, L.in, L.stride, L.hist, L.p, L.wbE, L.wbmeta, L.dm, K, nch, ns, nsamp, stream);
+	case CHAN_WB_REAL: return launch_channelize_wb_real(L.in, L.stride, L.hist.hpad, L.p, L.wbE, L.wbmeta, L.dm, K, nch, ns, nsamp, stream);
+	case CHAN_EXACT:
+	case CHAN_GENERIC: break;
+	}
+	const int blocks = L.form == CHAN_EXACT ? (int)(nrows / OUTBLK) : 0;
+	if (blocks) {
+		launched++;
+		if (int e = launch_channelize(L.in_kind, L.in, L.stride, L.wf, L.dm, K, L.taps_pad, nch, ns, blocks, nsamp, L.hist, stream)) return e;
+	}
+	const size_t row0 = (size_t)blocks * OUTBLK;
+	if (nrows == row0) return 0;
+	launched++;
+	return L.hist.hpad ? launch_channelize_generic_ovl(L.in_kind, L.in, L.stride, L.wf, L.dm, K, L.taps_pad, nch, ns, row0, nrows - row0,
+	                                                   nsamp, L.hist, stream)
+	                   : launch_channelize_generic(L.in_kind, L.in, L.stride, L.wf, L.dm, K, L.taps_pad, nch, ns, row0, nrows - row0, nsamp,
+	                                               stream);
+}
+
+/* Per stream the tables are wf [grp][taps_pad][8] (c, d), tw [grp][8][K/4] (Tr, Ti), twmeta [grp] and wbmeta [channel
+ * tile][WB_META], as the kernels above read them; p and the E tables serve every stream. */
+ChanLaunch chan_stream(const ChanLaunch &L, int s, unsigned long long pos0)
+{
+	const size_t ngrp = (L.nch + CH_GROUP - 1) / CH_GROUP, nctile = (L.nch + WB_CTILE - 1) / WB_CTILE;
+	ChanLaunch o = L;
+	o.in += s * L.stride;
+	o.hist.base = (const uint8_t *)L.hist.base + s * L.hist.stride;
+	o.hist.pos0 = pos0;
+	o.dm += s * L.nsamp * L.nch;
+	o.wf += s * ngrp * L.taps_pad * CH_GROUP * 2;
+	if (L.tw) o.tw += s * ngrp * CH_GROUP * (L.K / 4) * 2;
+	if (L.twmeta) o.twmeta += s * ngrp;
+	if (L.wbmeta) o.wbmeta += s * nctile * WB_META;
+	o.nstreams = 1;
+	return o;
 }
 
 /* ------------------------------------------------------------------------------------------
