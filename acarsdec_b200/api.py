@@ -20,6 +20,7 @@ TXTMAX = 250
 FLAG_FAST_WIDEBAND = 64          # ACB_FLAG_FAST_WIDEBAND: the fast forms for any K % 8 == 0 and any channel count
 FLAG_FAST_WIDEBAND_REAL = 128    # ACB_FLAG_FAST_WIDEBAND_REAL: the same for real input (air.c)
 FLAG_DECODE_STATS = 256          # ACB_FLAG_DECODE_STATS: per-chain decode statistics (Context.decode_stats)
+FLAG_LEVEL_STATS = 512           # ACB_FLAG_LEVEL_STATS: input and envelope levels (Context.level_stats)
 
 
 class Config(C.Structure):
@@ -93,6 +94,14 @@ DECODE_STATS_FIELDS = ("preamble", "started", "txt_parity", "txt_long", "txt_mis
                        "fec_short", "fec_parity_excess", "fec_parity", "fec_crc", "fec_fixed", "fec_unfixable",
                        "fec_parity_problem", "delivered", "lost")
 DECODE_STATS_DTYPE = np.dtype([(f, "<u8") for f in DECODE_STATS_FIELDS])
+
+# acb_input_level_t and acb_chan_level_t (include/acars_b200.h defines each field)
+INPUT_LEVEL_DTYPE = np.dtype([("samples", "<u8"), ("clipped", "<u8"), ("power_sum", "<f8"), ("peak", "<f4"), ("pad", "<f4")])
+CHAN_LEVEL_DTYPE = np.dtype([("rows", "<u8"), ("power_sum", "<f8"), ("peak", "<f4"), ("pad", "<f4"), ("windows", "<u8"),
+                             ("floor", "<f8")])
+# full-scale amplitude of each input kind's converted components: the mean input power in dBFS is
+# 10*log10(power_sum / samples / fs**2)
+FULL_SCALE = {"u8": 127.5, "cs16": 32768.0, "real": 1.0}
 
 
 # every symbol include/acars_b200.h declares: (name, restype, argtypes)
@@ -191,6 +200,8 @@ ABI = [
     ("acb_get_stats", C.c_int, [C.c_void_p, C.POINTER(Stats), C.c_int]),
     ("acb_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_multi_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_multi_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_block_fec", C.c_int, [C.POINTER(Msg)]),
     ("acb_block_fec_batch", C.c_int, [C.c_void_p, C.POINTER(Msg), C.c_int, C.POINTER(C.c_int)]),
     ("acb_crc_update", C.c_uint16, [C.c_uint16, C.c_uint8]),
@@ -705,6 +716,14 @@ class Context:
         _check(self.lib, self.lib.acb_get_decode_stats(self.h, out.ctypes.data, out.size, int(reset)))
         return out
 
+    def level_stats(self, reset: bool = False) -> tuple[np.ndarray, np.ndarray]:
+        """Input and envelope levels (FLAG_LEVEL_STATS): an INPUT_LEVEL_DTYPE array of shape (nstreams,) and a
+        CHAN_LEVEL_DTYPE array of shape (nstreams, nch)."""
+        inp = np.zeros(self.nstreams, dtype=INPUT_LEVEL_DTYPE)
+        ch = np.zeros((self.nstreams, self.nch), dtype=CHAN_LEVEL_DTYPE)
+        _check(self.lib, self.lib.acb_get_level_stats(self.h, inp.ctypes.data, inp.size, ch.ctypes.data, ch.size, int(reset)))
+        return inp, ch
+
     def device_alloc(self, nbytes: int) -> int:
         p = self.lib.acb_device_alloc(self.h, nbytes)
         if not p:
@@ -849,6 +868,19 @@ class MultiContext:
         out = np.zeros((self.nstreams, self.nch), dtype=DECODE_STATS_DTYPE)
         _check(self.lib, self.lib.acb_multi_get_decode_stats(self.h, out.ctypes.data, out.size, int(reset)))
         return out
+
+    def level_stats(self, reset: bool = False) -> tuple[np.ndarray, np.ndarray]:
+        """As Context.level_stats, indexed by global stream and channel (a channel split's input levels are part 0's)."""
+        inp = np.zeros(self.nstreams, dtype=INPUT_LEVEL_DTYPE)
+        ch = np.zeros((self.nstreams, self.nch), dtype=CHAN_LEVEL_DTYPE)
+        _check(self.lib, self.lib.acb_multi_get_level_stats(self.h, inp.ctypes.data, inp.size, ch.ctypes.data, ch.size, int(reset)))
+        return inp, ch
+
+    def part_input_levels(self, i: int) -> np.ndarray:
+        """The input table of the i-th per-device context: its streams first (in a channel split, every stream)."""
+        inp = np.zeros(self.nstreams, dtype=INPUT_LEVEL_DTYPE)
+        _check(self.lib, self.lib.acb_get_level_stats(self.lib.acb_multi_part(self.h, i), inp.ctypes.data, inp.size, None, 0, 0))
+        return inp
 
     def sync(self) -> int:
         return _check(self.lib, self.lib.acb_multi_sync(self.h))

@@ -155,6 +155,23 @@ int launch_move_tail(const uint32_t *src, uint32_t *dst, size_t stride, int K, i
                      int nstreams, CUstream_st *stream);
 int launch_hist_gather(const uint8_t *in, size_t stride, size_t blk_bytes, const int *nblk, uint8_t *hist, int hb, int nstreams,
                        CUstream_st *stream);
+/* ACB_FLAG_LEVEL_STATS.  k_level_in: one CTA per LVL_CHUNK input bytes of a stream, its partial (u8: clipped, sum of the
+ * bytes, sum of their squares; CS16: clipped, -, sum of I^2 + Q^2; real: clipped, -, the float64 sum of x^2 in m2's bits)
+ * to part[s * part_stride + chunk]; a final pass adds each stream's partials in chunk order into out[s].  k_level_dm: one
+ * CTA per (stream, 1024-row window, channel tile), each window's partial sum and peak per channel to
+ * seg_sum / seg_peak[(s * seg_stride + j) * nch + c]; a final pass per chain adds them in window order, closes the windows
+ * with the chain's open-window carry and writes out[s * nch + c].  `rows` != NULL (device array): the ragged form, stream
+ * s counts its first rows[s] <= nrows rows.  Both add the kernels they launch to `launched`; they return a cudaError_t. */
+constexpr int LVL_CHUNK = 256 * 16 * 8;
+struct LevelPart { unsigned long long clipped, m1, m2; float peak; unsigned pad; };
+struct LevelCarry { double sum; int rows; int pad; };    /* a chain's open window: its rows so far and their sum of dm^2 */
+/* one submit's results, laid out as acb_input_level_t and acb_chan_level_t (context.cu checks it) */
+struct LevelIn { unsigned long long samples, clipped; double power_sum; float peak, pad; };
+struct LevelChan { unsigned long long rows; double power_sum; float peak, pad; unsigned long long windows; double floor; };
+int launch_level_input(int in_kind, const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nstreams,
+                       LevelPart *part, size_t part_stride, LevelIn *out, CUstream_st *stream, int &launched);
+int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int nstreams, double *seg_sum, float *seg_peak,
+                    int seg_stride, LevelCarry *carry, LevelChan *out, CUstream_st *stream, int &launched);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
 

@@ -139,7 +139,7 @@ struct acb_ctx {
 	std::deque<Batch> outq;
 	size_t outq_count;
 	/* consumer thread: everything from `outq` to `jobs_done`, plus stats.raw_frames / fec_dropped, is guarded by mtx */
-	struct Job { Groups groups; int ring; unsigned count; unsigned long long seq; };
+	struct Job { Groups groups; int ring; unsigned count; unsigned long long seq; bool chan; };
 	std::thread consumer;
 	std::mutex mtx;
 	std::condition_variable cv_job, cv_done;
@@ -180,6 +180,22 @@ struct acb_ctx {
 	unsigned *h_evcnt[NPIPE];    /* pinned */
 	std::vector<acb_decode_stats_t> dstats;      /* guarded by dstats_mtx */
 	std::vector<unsigned long long> dstats_from; /* per stream: the first submit its counts cover (acb_reset_stream); dstats_mtx */
+	/* ACB_FLAG_LEVEL_STATS: per frame ring (submit in flight), the submit's input and envelope levels, written whole by the
+	 * level kernels on the channelizer stream (behind K1) and read back with that submit's frames; the consumer adds them to
+	 * lin / lch.  The open windows' carry (d_lcarry) is device state in submit order, on the channelizer stream. */
+	bool level_stats;
+	std::mutex lstats_mtx;       /* guards lin, lch, lstats_from */
+	LevelIn *d_lin[NPIPE], *h_lin[NPIPE];         /* [stream] (h_* pinned) */
+	LevelChan *d_lch[NPIPE], *h_lch[NPIPE];       /* [chain] */
+	cudaEvent_t ev_lvl_done[NPIPE];               /* behind the level kernels of the submit using ring b */
+	LevelPart *d_lpart;                           /* k_level_in's per-chunk partials, [stream][lpart_stride] */
+	size_t lpart_stride;
+	double *d_lseg_sum;                           /* k_level_dm's per-window partials, [stream][max_blocks + 2][nch] */
+	float *d_lseg_peak;
+	LevelCarry *d_lcarry;                         /* [chain] */
+	std::vector<acb_input_level_t> lin;           /* guarded by lstats_mtx */
+	std::vector<acb_chan_level_t> lch;
+	std::vector<unsigned long long> lstats_from;  /* per stream: the first submit its levels cover (acb_reset_stream) */
 	int *d_rag[NRAG], *h_rag[NRAG];               /* ragged submits' counts (h_rag pinned) */
 	cudaEvent_t ev_rag_used[NRAG][3];             /* behind the last reads of slot i on the copy, channelizer and demod streams */
 	bool rag_used[NRAG];
@@ -276,6 +292,13 @@ static int reset_states(acb_ctx *c)
 		std::lock_guard<std::mutex> lk(c->dstats_mtx);
 		memset(c->dstats.data(), 0, c->dstats.size() * sizeof(acb_decode_stats_t));
 	}
+	if (c->level_stats) {        /* the windows restart with the streams */
+		CU(cudaMemsetAsync(c->d_lcarry, 0, c->lch.size() * sizeof(LevelCarry), c->s_copy));
+		CU(cudaStreamSynchronize(c->s_copy));
+		std::lock_guard<std::mutex> lk(c->lstats_mtx);
+		memset(c->lin.data(), 0, c->lin.size() * sizeof(acb_input_level_t));
+		memset(c->lch.data(), 0, c->lch.size() * sizeof(acb_chan_level_t));
+	}
 	c->overflowed = false;
 	return ACB_OK;
 }
@@ -351,6 +374,12 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	for (int i = 0; i < NRAG; i++) c->d_rag[i] = nullptr, c->h_rag[i] = nullptr;
 	c->decode_stats = (cfg->flags & ACB_FLAG_DECODE_STATS) != 0;
 	for (int i = 0; i < NPIPE; i++) c->d_evcnt[i] = nullptr, c->h_evcnt[i] = nullptr;
+	c->level_stats = (cfg->flags & ACB_FLAG_LEVEL_STATS) != 0;
+	for (int i = 0; i < NPIPE; i++) c->d_lin[i] = c->h_lin[i] = nullptr, c->d_lch[i] = c->h_lch[i] = nullptr, c->ev_lvl_done[i] = nullptr;
+	c->d_lpart = nullptr;
+	c->d_lseg_sum = nullptr;
+	c->d_lseg_peak = nullptr;
+	c->d_lcarry = nullptr;
 	*out = c;
 
 	{
@@ -480,6 +509,31 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 			CU(cudaHostAlloc(&c->h_evcnt[i], nchain * EV_COUNT * sizeof(unsigned), cudaHostAllocDefault));
 		}
 	}
+	if (c->level_stats) {
+		static_assert(sizeof(LevelIn) == sizeof(acb_input_level_t) && offsetof(LevelIn, peak) == offsetof(acb_input_level_t, peak),
+		              "LevelIn is acb_input_level_t");
+		static_assert(sizeof(LevelChan) == sizeof(acb_chan_level_t) && offsetof(LevelChan, floor) == offsetof(acb_chan_level_t, floor),
+		              "LevelChan is acb_chan_level_t");
+		const int ns = cfg->nstreams;
+		c->lin.assign(ns, acb_input_level_t{});
+		c->lch.assign(nchain, acb_chan_level_t{});
+		c->lstats_from.assign(ns, 0);
+		for (int i = 0; i < NPIPE; i++) {
+			CU(cudaMalloc(&c->d_lin[i], ns * sizeof(LevelIn)));
+			CU(cudaHostAlloc(&c->h_lin[i], ns * sizeof(LevelIn), cudaHostAllocDefault));
+			CU(cudaMalloc(&c->d_lch[i], nchain * sizeof(LevelChan)));
+			CU(cudaHostAlloc(&c->h_lch[i], nchain * sizeof(LevelChan), cudaHostAllocDefault));
+			CU(cudaEventCreateWithFlags(&c->ev_lvl_done[i], cudaEventDisableTiming));
+		}
+		/* a stream's rows of one submit: at most max_blocks * 1024 rows of K samples */
+		const size_t in_bytes_max = (size_t)cfg->max_blocks * OUTBLK * cfg->K * (c->in_kind == IN_KIND_U8IQ ? 2 : 4);
+		c->lpart_stride = (in_bytes_max + LVL_CHUNK - 1) / LVL_CHUNK;
+		CU(cudaMalloc(&c->d_lpart, (size_t)ns * c->lpart_stride * sizeof(LevelPart)));
+		const size_t nseg = (size_t)ns * (cfg->max_blocks + 2) * cfg->nch;
+		CU(cudaMalloc(&c->d_lseg_sum, nseg * sizeof(double)));
+		CU(cudaMalloc(&c->d_lseg_peak, nseg * sizeof(float)));
+		CU(cudaMalloc(&c->d_lcarry, nchain * sizeof(LevelCarry)));
+	}
 	c->rag_seq = 0;
 	for (int i = 0; i < NRAG; i++) {
 		CU(cudaMalloc(&c->d_rag[i], 4 * (size_t)cfg->nstreams * sizeof(int)));
@@ -536,7 +590,10 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 			cudaEventDestroy(c->ev_k2_done[i]); cudaEventDestroy(c->ev_ring_read[i]);
 			cudaFree(c->d_ring[i]); cudaFree(c->d_ctl[i]); cudaFreeHost(c->h_ctl[i]); cudaFreeHost(c->h_ring[i]);
 			cudaFree(c->d_evcnt[i]); cudaFreeHost(c->h_evcnt[i]);
+			cudaFree(c->d_lin[i]); cudaFreeHost(c->h_lin[i]); cudaFree(c->d_lch[i]); cudaFreeHost(c->h_lch[i]);
+			if (c->ev_lvl_done[i]) cudaEventDestroy(c->ev_lvl_done[i]);
 		}
+		cudaFree(c->d_lpart); cudaFree(c->d_lseg_sum); cudaFree(c->d_lseg_peak); cudaFree(c->d_lcarry);
 		for (int i = 0; i < NRAG; i++) {
 			if (!c->d_rag[i]) continue;
 			cudaFree(c->d_rag[i]); cudaFreeHost(c->h_rag[i]);
@@ -587,6 +644,14 @@ extern "C" int acb_reset_stream(acb_ctx_t *c, int stream)
 		std::lock_guard<std::mutex> lk(c->dstats_mtx);
 		memset(&c->dstats[(size_t)stream * c->cfg.nch], 0, (size_t)c->cfg.nch * sizeof(acb_decode_stats_t));
 		c->dstats_from[stream] = c->nsubmit;
+	}
+	if (c->level_stats) {
+		/* the stream's open windows, behind the level kernels already queued on the channelizer stream */
+		CU(cudaMemsetAsync(c->d_lcarry + (size_t)stream * c->cfg.nch, 0, (size_t)c->cfg.nch * sizeof(LevelCarry), c->s_comp));
+		std::lock_guard<std::mutex> lk(c->lstats_mtx);
+		c->lin[stream] = acb_input_level_t{};
+		memset(&c->lch[(size_t)stream * c->cfg.nch], 0, (size_t)c->cfg.nch * sizeof(acb_chan_level_t));
+		c->lstats_from[stream] = c->nsubmit;
 	}
 	return ACB_OK;
 }
@@ -762,6 +827,34 @@ static void add_decode_stats(acb_ctx *c, const acb_ctx::Job &job, const RawFrame
 	}
 }
 
+/* ACB_FLAG_LEVEL_STATS: a collected submit's levels into the context's tables (envelope input has no input levels) */
+static void add_level_stats(acb_ctx *c, const acb_ctx::Job &job)
+{
+	std::lock_guard<std::mutex> lk(c->lstats_mtx);
+	const int nch = c->cfg.nch;
+	const LevelIn *in = c->h_lin[job.ring];
+	const LevelChan *ch = c->h_lch[job.ring];
+	for (int s = 0; s < c->cfg.nstreams; s++) {
+		if (job.seq < c->lstats_from[s]) continue;        /* made before the stream's acb_reset_stream */
+		if (job.chan) {
+			acb_input_level_t &d = c->lin[s];
+			d.samples += in[s].samples;
+			d.clipped += in[s].clipped;
+			d.power_sum += in[s].power_sum;
+			d.peak = std::max(d.peak, in[s].peak);
+		}
+		for (int k = 0; k < nch; k++) {
+			const LevelChan &e = ch[(size_t)s * nch + k];
+			acb_chan_level_t &d = c->lch[(size_t)s * nch + k];
+			d.rows += e.rows;
+			d.power_sum += e.power_sum;
+			d.peak = std::max(d.peak, e.peak);
+			if (e.windows) d.floor = d.windows ? std::min(d.floor, e.floor) : e.floor;
+			d.windows += e.windows;
+		}
+	}
+}
+
 static void consume(acb_ctx *c, const acb_ctx::Job &job)
 {
 	const unsigned count = job.count;
@@ -896,6 +989,7 @@ static void consume(acb_ctx *c, const acb_ctx::Job &job)
 		for (auto &th : pool) th.join();
 	}
 	if (c->decode_stats) add_decode_stats(c, job, ring, keep.data());     /* before the job counts as done */
+	if (c->level_stats) add_level_stats(c, job);
 	const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
 	std::lock_guard<std::mutex> lk(c->mtx);
 	c->stats.raw_frames += count;
@@ -919,7 +1013,7 @@ static void consumer_main(acb_ctx *c)
 			job = std::move(c->jobs.front());
 			c->jobs.pop_front();
 		}
-		const cudaError_t e = job.count || c->decode_stats ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
+		const cudaError_t e = job.count || c->decode_stats || c->level_stats ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
 		if (e == cudaSuccess) consume(c, job);
 		{
 			std::lock_guard<std::mutex> lk(c->mtx);
@@ -966,11 +1060,16 @@ static int harvest_begin(acb_ctx *c)
 	if (c->decode_stats)           /* the submit's demod is done (ev.c follows it): its counters travel with its frames */
 		CU(cudaMemcpyAsync(c->h_evcnt[t.ring], c->d_evcnt[t.ring], c->dstats.size() * EV_COUNT * sizeof(unsigned),
 		                   cudaMemcpyDeviceToHost, c->s_d2h));
+	if (c->level_stats) {          /* the level kernels run on the channelizer stream: the copies wait for them */
+		CU(cudaStreamWaitEvent(c->s_d2h, c->ev_lvl_done[t.ring], 0));
+		CU(cudaMemcpyAsync(c->h_lin[t.ring], c->d_lin[t.ring], c->lin.size() * sizeof(LevelIn), cudaMemcpyDeviceToHost, c->s_d2h));
+		CU(cudaMemcpyAsync(c->h_lch[t.ring], c->d_lch[t.ring], c->lch.size() * sizeof(LevelChan), cudaMemcpyDeviceToHost, c->s_d2h));
+	}
 	CU(cudaEventRecord(c->ev_ring_read[t.ring], c->s_d2h));
 	c->ring_read_pending[t.ring] = true;
 	{
 		std::lock_guard<std::mutex> lk(c->mtx);
-		c->jobs.push_back(acb_ctx::Job{ std::move(t.groups), t.ring, count, t.seq });
+		c->jobs.push_back(acb_ctx::Job{ std::move(t.groups), t.ring, count, t.seq, t.ev.chan });
 		c->ring_job[t.ring] = ++c->jobs_queued;
 	}
 	c->cv_job.notify_one();
@@ -983,6 +1082,25 @@ static int collect_oldest(acb_ctx *c)
 	if (int r = harvest_begin(c)) return r;
 	wait_consumer(c, c->jobs_queued);
 	if (c->consumer_err[0]) return fail(ACB_ERR_CUDA, "%s", c->consumer_err);
+	return ACB_OK;
+}
+
+/* ACB_FLAG_LEVEL_STATS: the levels of the submit using ring b, on the channelizer stream: the input's (`in`, NULL for
+ * envelope input) and the envelope's.  They write that ring's result buffers, so they wait until the read-back of the
+ * submit that used it before is done. */
+static int run_level(acb_ctx *c, int b, const uint8_t *in, size_t stride, int nsamp, const int *rag)
+{
+	if (c->ring_read_pending[b]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_ring_read[b], 0));
+	int launched = 0;
+	int r = in ? launch_level_input(c->in_kind, in, stride, c->cfg.K, nsamp, rag, c->cfg.nstreams, c->d_lpart, c->lpart_stride, c->d_lin[b],
+	                                c->s_comp, launched)
+	           : 0;
+	if (!r)
+		r = launch_level_dm(c->d_dm[b], nsamp, rag, c->cfg.nch, c->cfg.nstreams, c->d_lseg_sum, c->d_lseg_peak, c->cfg.max_blocks + 2,
+		                    c->d_lcarry, c->d_lch[b], c->s_comp, launched);
+	c->stats.kernel_launches += launched;
+	if (r) return fail(ACB_ERR_CUDA, "level launch: %s", cudaGetErrorString((cudaError_t)r));
+	CU(cudaEventRecord(c->ev_lvl_done[b], c->s_comp));
 	return ACB_OK;
 }
 
@@ -1077,10 +1195,24 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		CU(cudaEventRecord(c->ev_k1_done[b], c->s_comp));
 		c->k1_pending[b] = true;
 		CU(cudaStreamWaitEvent(c->s_dem, c->ev_k1_done[b], 0));
+		if (c->level_stats) {
+			/* behind K1, beside the demod; the input-lifetime event moves behind them, as they read the input too */
+			if (int r2 = run_level(c, b, d_iq, stride, nsamp, rag)) return r2;
+			CU(cudaEventRecord(c->ev_k1_done[b], c->s_comp));
+		}
 	} else if (dm_host) {
 		/* envelope input: the copy is ordered behind the previous demod on the same stream, and
 		 * behind any channelizer launch that still targets the other buffer only */
+		if (c->level_stats) {      /* and behind the level kernels, which may still read this buffer */
+			CU(cudaEventRecord(c->ev_join, c->s_comp));
+			CU(cudaStreamWaitEvent(c->s_dem, c->ev_join, 0));
+		}
 		CU(cudaMemcpyAsync(dmbuf, dm_host, (size_t)c->cfg.nstreams * nsamp * c->cfg.nch * sizeof(float), cudaMemcpyHostToDevice, c->s_dem));
+		if (c->level_stats) {
+			CU(cudaEventRecord(c->ev_join, c->s_dem));
+			CU(cudaStreamWaitEvent(c->s_comp, c->ev_join, 0));
+			if (int r2 = run_level(c, b, nullptr, 0, nsamp, nullptr)) return r2;
+		}
 	}
 	if (c->ring_read_pending[b]) {
 		CU(cudaStreamWaitEvent(c->s_dem, c->ev_ring_read[b], 0));
@@ -1856,5 +1988,21 @@ extern "C" int acb_get_decode_stats(acb_ctx_t *c, acb_decode_stats_t *out, size_
 	std::lock_guard<std::mutex> lk(c->dstats_mtx);
 	memcpy(out, c->dstats.data(), c->dstats.size() * sizeof(acb_decode_stats_t));
 	if (reset) memset(c->dstats.data(), 0, c->dstats.size() * sizeof(acb_decode_stats_t));
+	return ACB_OK;
+}
+
+extern "C" int acb_get_level_stats(acb_ctx_t *c, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset)
+{
+	if (!c) return fail(ACB_ERR_ARG, "null context");
+	if (!c->level_stats) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_LEVEL_STATS");
+	if (in && n_in < c->lin.size()) return fail(ACB_ERR_ARG, "n_in=%zu < nstreams=%zu", n_in, c->lin.size());
+	if (ch && n_ch < c->lch.size()) return fail(ACB_ERR_ARG, "n_ch=%zu < nstreams*nch=%zu", n_ch, c->lch.size());
+	std::lock_guard<std::mutex> lk(c->lstats_mtx);
+	if (in) memcpy(in, c->lin.data(), c->lin.size() * sizeof(acb_input_level_t));
+	if (ch) memcpy(ch, c->lch.data(), c->lch.size() * sizeof(acb_chan_level_t));
+	if (reset) {                 /* the open windows stay on the device: the alignment is kept */
+		memset(c->lin.data(), 0, c->lin.size() * sizeof(acb_input_level_t));
+		memset(c->lch.data(), 0, c->lch.size() * sizeof(acb_chan_level_t));
+	}
 	return ACB_OK;
 }

@@ -3607,4 +3607,273 @@ int launch_block_fec_stats(RawFrame *ring, const RingCtl *ctl, unsigned cap, cud
 	return (int)cudaGetLastError();
 }
 
+/* ---- ACB_FLAG_LEVEL_STATS: input and envelope levels (launch_level_input, launch_level_dm) ----
+ * Memory-bound reductions over what a submit already holds.  Integer counts and sums are exact in any order; the float64
+ * sums are made in a fixed order (each thread in address order, then fixed trees, then the partials in chunk / window
+ * order), so the same input with the same cuts gives the same bits.  No floating-point atomics. */
+constexpr int LVL_THREADS = 256;
+
+/* one thread's share of a chunk of input words (4 bytes: two u8 samples, one CS16 sample or one real sample) */
+template <int KIND> struct LevelAcc {
+	unsigned clip = 0;
+	unsigned long long m1 = 0, m2 = 0;            /* u8: sum of the bytes, of their squares; CS16: -, sum of I^2 + Q^2 */
+	double p = 0.0;                               /* real: sum of x^2 */
+	unsigned hi = 0, lo = 0xffffffffu;            /* u8: per-byte max / min; CS16: hi = largest |component| */
+	float pk = 0.0f;                              /* real: largest |x| */
+	__device__ __forceinline__ void add(unsigned w)
+	{
+		if (KIND == IN_U8IQ) {
+			/* a thread sees at most 8 * 4 words per chunk: the byte sums stay far below 2^32 */
+			m1 = __dp4a(w, 0x01010101u, (unsigned)m1);
+			m2 = __dp4a(w, w, (unsigned)m2);
+			/* a byte is 0 or 255 exactly when its 8 bits are equal: b ^ (b >> 1) has no bit set in 0..6 */
+			const unsigned u = (w ^ (w >> 1)) & 0x7f7f7f7fu, z = ~((u + 0x7f7f7f7fu) | u) & 0x80808080u;
+			clip += ((z & 0x00008080u) != 0) + ((z & 0x80800000u) != 0);
+			hi = __vmaxu4(hi, w);
+			lo = __vminu4(lo, w);
+		} else if (KIND == IN_CS16IQ) {
+			const int i = (int)(short)(w & 0xffffu), q = (int)w >> 16;
+			m2 += (unsigned)(i * i) + (unsigned)(q * q);
+			clip += (i == -32768) | (i == 32767) | (q == -32768) | (q == 32767);
+			hi = max(hi, (unsigned)max(abs(i), abs(q)));
+		} else {
+			const float x = __uint_as_float(w);
+			const double xd = (double)x;
+			p = __dadd_rn(p, __dmul_rn(xd, xd));
+			clip += (x <= -1.0f) | (x >= 2047.0f / 2048.0f);
+			pk = fmaxf(pk, fabsf(x));
+		}
+	}
+	__device__ __forceinline__ LevelPart part() const
+	{
+		LevelPart r;
+		r.clipped = clip;
+		r.m1 = m1;
+		r.m2 = KIND == IN_F32REAL ? (unsigned long long)__double_as_longlong(p) : m2;
+		if (KIND == IN_U8IQ) {
+			unsigned bmax = 0, bmin = 255;
+			for (int k = 0; k < 4; k++) bmax = max(bmax, (hi >> (8 * k)) & 0xffu), bmin = min(bmin, (lo >> (8 * k)) & 0xffu);
+			/* |(float)b - 127.37f| is exact: the difference of the two floats has at most 24 significant bits */
+			r.peak = fmaxf(0.0f, fmaxf((float)bmax - 127.37f, 127.37f - (float)bmin));
+		} else {
+			r.peak = KIND == IN_CS16IQ ? (float)hi : pk;
+		}
+		r.pad = 0;
+		return r;
+	}
+};
+
+/* partials a, b into a (integers add exactly; the real kind's float64 sum in m2's bits) */
+template <int KIND> __device__ __forceinline__ void level_merge(LevelPart &a, const LevelPart &b)
+{
+	a.clipped += b.clipped;
+	a.m1 += b.m1;
+	a.m2 = KIND == IN_F32REAL ? (unsigned long long)__double_as_longlong(__dadd_rn(__longlong_as_double((long long)a.m2),
+	                                                                               __longlong_as_double((long long)b.m2)))
+	                          : a.m2 + b.m2;
+	a.peak = fmaxf(a.peak, b.peak);
+}
+
+template <int KIND> __device__ __forceinline__ void level_shfl_merge(LevelPart &v, int lane_mask)
+{
+	LevelPart o;
+	o.clipped = __shfl_xor_sync(0xffffffffu, v.clipped, lane_mask);
+	o.m1 = __shfl_xor_sync(0xffffffffu, v.m1, lane_mask);
+	o.m2 = __shfl_xor_sync(0xffffffffu, v.m2, lane_mask);
+	o.peak = __shfl_xor_sync(0xffffffffu, v.peak, lane_mask);
+	level_merge<KIND>(v, o);                      /* the butterfly adds the same two values in every lane: a + b == b + a */
+}
+
+/* bytes of input per sample (u8: I, Q bytes; CS16: I, Q int16; real: one float) */
+template <int KIND> __host__ __device__ constexpr int level_sample_bytes() { return KIND == IN_U8IQ ? 2 : 4; }
+
+/* grid (chunk, stream): stream s's rows*K samples at in + s*stride, LVL_CHUNK bytes per CTA, 16-byte loads (the rows start
+ * 16-byte aligned; a streaming kind's last few words, when rows*K is not a multiple of 4, go one by one) */
+template <int KIND>
+__global__ void __launch_bounds__(LVL_THREADS)
+k_level_in(const uint8_t *__restrict__ in, size_t stride, int K, int nrows, const int *__restrict__ rows, LevelPart *__restrict__ part,
+           size_t part_stride)
+{
+	const int s = blockIdx.y;
+	const size_t bytes = (size_t)(rows ? rows[s] : nrows) * K * level_sample_bytes<KIND>();
+	const size_t c0 = (size_t)blockIdx.x * LVL_CHUNK;
+	if (c0 >= bytes) return;
+	const size_t c1 = min(bytes, c0 + LVL_CHUNK);
+	const uint8_t *base = in + (size_t)s * stride;
+	LevelAcc<KIND> a;
+	const size_t v1 = c0 + (c1 - c0) / 16 * 16;
+#pragma unroll 4
+	for (size_t o = c0 + 16 * (size_t)threadIdx.x; o < v1; o += 16 * LVL_THREADS) {
+		const uint4 w = __ldcs(reinterpret_cast<const uint4 *>(base + o));       /* read once: do not keep it in L2 */
+		a.add(w.x); a.add(w.y); a.add(w.z); a.add(w.w);
+	}
+	for (size_t o = v1 + 4 * (size_t)threadIdx.x; o < c1; o += 4 * LVL_THREADS) a.add(*reinterpret_cast<const unsigned *>(base + o));
+	LevelPart v = a.part();
+	for (int m = 16; m; m >>= 1) level_shfl_merge<KIND>(v, m);
+	__shared__ LevelPart s_w[LVL_THREADS / 32];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	if (lane == 0) s_w[warp] = v;
+	__syncthreads();
+	if (warp == 0) {
+		v = s_w[lane < LVL_THREADS / 32 ? lane : 0];
+		if (lane >= LVL_THREADS / 32) v = LevelPart{ 0, 0, 0, 0.0f, 0 };   /* the real kind's +0.0 has all bits zero */
+		for (int m = 16; m; m >>= 1) level_shfl_merge<KIND>(v, m);
+		if (lane == 0) part[(size_t)s * part_stride + blockIdx.x] = v;
+	}
+}
+
+/* one warp per stream: its chunks' partials in a fixed order (lane l takes chunks l, l + 32, ..., then a butterfly) */
+template <int KIND>
+__global__ void __launch_bounds__(256)
+k_level_in_fin(int K, int nrows, const int *__restrict__ rows, int nstreams, const LevelPart *__restrict__ part, size_t part_stride,
+               LevelIn *__restrict__ out)
+{
+	const int s = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+	if (s >= nstreams) return;
+	const unsigned long long samples = (unsigned long long)(rows ? rows[s] : nrows) * (unsigned long long)K;
+	const size_t nchunk = (samples * level_sample_bytes<KIND>() + LVL_CHUNK - 1) / LVL_CHUNK;
+	LevelPart v{ 0, 0, 0, 0.0f, 0 };
+	for (size_t j = lane; j < nchunk; j += 32) level_merge<KIND>(v, part[(size_t)s * part_stride + j]);
+	for (int m = 16; m; m >>= 1) level_shfl_merge<KIND>(v, m);
+	if (lane) return;
+	double p;
+	if (KIND == IN_U8IQ) {
+		/* components v = (b - 127) - d with d = 127.37f - 127 (exact, 16 significant bits):
+		 * sum v^2 = sum (b-127)^2 - 2 d sum (b-127) + N d^2, the two sums exact integers */
+		const unsigned long long n = 2 * samples;
+		const long long s1 = (long long)v.m1 - 127 * (long long)n;
+		const unsigned long long s2 = v.m2 + 16129ull * n - 254ull * v.m1;
+		const double d = (double)(127.37f - 127.0f);
+		p = __dadd_rn(__dsub_rn((double)s2, __dmul_rn(2.0 * d, (double)s1)), __dmul_rn((double)n, __dmul_rn(d, d)));
+	} else {
+		p = KIND == IN_CS16IQ ? (double)v.m2 : __longlong_as_double((long long)v.m2);
+	}
+	out[s] = LevelIn{ samples, v.clipped, p, v.peak, 0.0f };
+}
+
+template <int KIND>
+static int launch_level_input_t(const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nstreams, LevelPart *part,
+                                size_t part_stride, LevelIn *out, cudaStream_t stream, int &launched)
+{
+	const size_t nchunk = ((size_t)nrows * K * level_sample_bytes<KIND>() + LVL_CHUNK - 1) / LVL_CHUNK;
+	if (nchunk == 0) return (int)cudaErrorInvalidValue;
+	k_level_in<KIND><<<dim3((unsigned)nchunk, nstreams), LVL_THREADS, 0, stream>>>(in, stride, K, nrows, rows, part, part_stride);
+	k_level_in_fin<KIND><<<(unsigned)((nstreams * 32 + 255) / 256), 256, 0, stream>>>(K, nrows, rows, nstreams, part, part_stride, out);
+	launched += 2;
+	return (int)cudaGetLastError();
+}
+
+int launch_level_input(int in_kind, const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nstreams, LevelPart *part,
+                       size_t part_stride, LevelIn *out, cudaStream_t stream, int &launched)
+{
+	if (in_kind == IN_KIND_U8IQ) return launch_level_input_t<IN_U8IQ>(in, stride, K, nrows, rows, nstreams, part, part_stride, out, stream, launched);
+	if (in_kind == IN_KIND_CS16IQ) return launch_level_input_t<IN_CS16IQ>(in, stride, K, nrows, rows, nstreams, part, part_stride, out, stream, launched);
+	return launch_level_input_t<IN_F32REAL>(in, stride, K, nrows, rows, nstreams, part, part_stride, out, stream, launched);
+}
+
+/* Window j of stream s in this submit: rows [lo, hi) with the stream's open window holding n0 rows, so that
+ * j * 1024 - n0 starts window j (the first one closes the open window) */
+__device__ __forceinline__ void level_window(int j, int n0, int rows, int &lo, int &hi)
+{
+	lo = max(0, j * OUTBLK - n0);
+	hi = min(rows, (j + 1) * OUTBLK - n0);
+}
+
+/* grid (window, stream, channel tile), LVL_THREADS threads as LVL_THREADS / ct row lanes x ct channels: each warp reads
+ * whole runs of dm[s][n][c] (channels contiguous), each thread its channel's rows in order, then a fixed tree over the
+ * row lanes */
+__global__ void __launch_bounds__(LVL_THREADS)
+k_level_dm(const float *__restrict__ dm, int nrows, const int *__restrict__ rows, int nch, int ct, const LevelCarry *__restrict__ carry,
+           double *__restrict__ seg_sum, float *__restrict__ seg_peak, int seg_stride)
+{
+	const int s = blockIdx.y, j = blockIdx.x;
+	int lo, hi;
+	level_window(j, carry[(size_t)s * nch].rows, rows ? rows[s] : nrows, lo, hi);
+	if (lo >= hi) return;
+	const int nl = LVL_THREADS / ct, r0 = threadIdx.x / ct, cc = threadIdx.x % ct, c = blockIdx.z * ct + cc;
+	double sum = 0.0;
+	float pk = 0.0f;
+	if (c < nch) {
+		const float *p = dm + (size_t)s * nrows * nch + c;
+#pragma unroll 4
+		for (int n = lo + r0; n < hi; n += nl) {
+			const float x = __ldcs(p + (size_t)n * nch);
+			const double xd = (double)x;
+			sum = __dadd_rn(sum, __dmul_rn(xd, xd));
+			pk = fmaxf(pk, x);
+		}
+	}
+	__shared__ double s_sum[LVL_THREADS];
+	__shared__ float s_pk[LVL_THREADS];
+	s_sum[threadIdx.x] = sum;
+	s_pk[threadIdx.x] = pk;
+	__syncthreads();
+	for (int h = nl / 2; h; h >>= 1) {
+		if (r0 < h) {
+			s_sum[threadIdx.x] = __dadd_rn(s_sum[threadIdx.x], s_sum[threadIdx.x + h * ct]);
+			s_pk[threadIdx.x] = fmaxf(s_pk[threadIdx.x], s_pk[threadIdx.x + h * ct]);
+		}
+		__syncthreads();
+	}
+	if (r0 == 0 && c < nch) {
+		const size_t o = ((size_t)s * seg_stride + j) * nch + c;
+		seg_sum[o] = s_sum[threadIdx.x];
+		seg_peak[o] = s_pk[threadIdx.x];
+	}
+}
+
+/* one thread per chain: its windows' partials in order; closed windows give their mean, the last open one becomes the
+ * carry */
+__global__ void __launch_bounds__(256)
+k_level_dm_fin(int nrows, const int *__restrict__ rows, int nch, int nstreams, LevelCarry *__restrict__ carry,
+               const double *__restrict__ seg_sum, const float *__restrict__ seg_peak, int seg_stride, LevelChan *__restrict__ out)
+{
+	const size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+	if (g >= (size_t)nstreams * nch) return;
+	const int s = (int)(g / nch), c = (int)(g % nch), n = rows ? rows[s] : nrows;
+	LevelCarry cr = carry[g];
+	const int n0 = cr.rows;                       /* the windows of this submit are placed by the carry it started with */
+	LevelChan r{ (unsigned long long)n, 0.0, 0.0f, 0.0f, 0, 0.0 };
+	const int nwin = n ? (n0 + n + OUTBLK - 1) / OUTBLK : 0;
+	for (int j = 0; j < nwin; j++) {
+		int lo, hi;
+		level_window(j, n0, n, lo, hi);
+		const size_t o = ((size_t)s * seg_stride + j) * nch + c;
+		const double x = seg_sum[o];
+		r.power_sum = __dadd_rn(r.power_sum, x);
+		r.peak = fmaxf(r.peak, seg_peak[o]);
+		const double w = j ? x : __dadd_rn(cr.sum, x);
+		const int wr = (j ? 0 : n0) + (hi - lo);
+		if (wr == OUTBLK) {
+			const double mean = w / OUTBLK;
+			r.floor = r.windows ? fmin(r.floor, mean) : mean;
+			r.windows++;
+			cr.sum = 0.0;
+			cr.rows = 0;
+		} else {
+			cr.sum = w;
+			cr.rows = wr;
+		}
+	}
+	carry[g] = cr;
+	out[g] = r;
+}
+
+int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int nstreams, double *seg_sum, float *seg_peak, int seg_stride,
+                    LevelCarry *carry, LevelChan *out, cudaStream_t stream, int &launched)
+{
+	/* channels per tile: the channel count rounded up to a power of two, at most a warp's worth */
+	int ct = 1;
+	while (ct < nch && ct < 32) ct *= 2;
+	const unsigned nwin = (unsigned)(nrows / OUTBLK + 2);                     /* an open window, whole ones, a new open one */
+	if (nwin > (unsigned)seg_stride) return (int)cudaErrorInvalidValue;
+	k_level_dm<<<dim3(nwin, nstreams, (nch + ct - 1) / ct), LVL_THREADS, 0, stream>>>(dm, nrows, rows, nch, ct, carry, seg_sum, seg_peak,
+	                                                                                  seg_stride);
+	const size_t nchain = (size_t)nstreams * nch;
+	k_level_dm_fin<<<(unsigned)((nchain + 255) / 256), 256, 0, stream>>>(nrows, rows, nch, nstreams, carry, seg_sum, seg_peak, seg_stride, out);
+	launched += 2;
+	return (int)cudaGetLastError();
+}
+
 } // namespace acb
+

@@ -425,3 +425,27 @@ extern "C" int acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *ou
 	}
 	return ACB_OK;
 }
+
+/* each part's tables at the global indices of its streams and chains; in a channel split every part reads every sample,
+ * and the input table is part 0's */
+extern "C" int acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset)
+{
+	if (!m) return fail(ACB_ERR_ARG, "null argument");
+	const int nch = m->cfg.nch;
+	if (in && n_in < (size_t)m->cfg.nstreams) return fail(ACB_ERR_ARG, "n_in=%zu < nstreams", n_in);
+	if (ch && n_ch < (size_t)m->cfg.nstreams * nch) return fail(ACB_ERR_ARG, "n_ch=%zu < nstreams*nch", n_ch);
+	std::vector<acb_input_level_t> pin;
+	std::vector<acb_chan_level_t> pch;
+	for (size_t i = 0; i < m->parts.size(); i++) {
+		const Part &p = m->parts[i];
+		pin.resize(p.ns);
+		pch.resize((size_t)p.ns * p.nc);
+		if (int r = acb_get_level_stats(p.ctx, pin.data(), pin.size(), pch.data(), pch.size(), reset)) return r;
+		if (in && (m->mode == ACB_MULTI_SPLIT_STREAMS || i == 0))
+			for (int s = 0; s < p.ns; s++) in[p.s0 + s] = pin[s];
+		if (ch)
+			for (int s = 0; s < p.ns; s++)
+				for (int c = 0; c < p.nc; c++) ch[(size_t)(p.s0 + s) * nch + p.c0 + c] = pch[(size_t)s * p.nc + c];
+	}
+	return ACB_OK;
+}

@@ -153,6 +153,12 @@ typedef struct {
                                          and channelizer form.  With this flag, ACB_DEMOD_LANES values other than 1, 2, 4 and
                                          8 are ignored and the picked default width runs (the other kernel forms have no
                                          counting form).  Without it acb_get_decode_stats returns ACB_ERR_ARG. */
+#define ACB_FLAG_LEVEL_STATS 512      /* keep per-stream input levels and per-chain envelope levels (acb_input_level_t,
+                                         acb_chan_level_t, acb_get_level_stats): input power, clipping and peak, channel
+                                         power, peak and noise floor, reduced on the device from the input and envelope
+                                         each submit already holds.  Any input kind and channelizer form, with or without
+                                         ACB_FLAG_DECODE_STATS; messages, envelope, chain states and decode statistics are
+                                         unchanged.  Without it acb_get_level_stats returns ACB_ERR_ARG. */
 
 /* One decoded block, after parity/CRC repair: msgblk_t (acarsdec.h:48-57) without the queue
  * link, plus where it came from.  `txt` is parity-stripped (acars.c:200). */
@@ -509,6 +515,41 @@ typedef struct {
  * without ACB_FLAG_DECODE_STATS. */
 int acb_get_decode_stats(acb_ctx_t *ctx, acb_decode_stats_t *out, size_t n, int reset);
 
+/* Levels (ACB_FLAG_LEVEL_STATS): how loud each receiver's input is and whether its ADC clips, and how much power and
+ * noise each channel's envelope carries — the receiver side of frames that were never started.
+ *
+ * Input, per stream.  The samples counted are, for every output row m a covered submit produced for the stream, the K
+ * input samples [m*K, (m+1)*K): each sample exactly once, whatever the cuts (a streaming kind's carried remainder counts
+ * when its row completes; the history of taps > K is not counted again).  A sample's components are converted as the
+ * channelizer converts them: u8 (float)b - 127.37f, CS16 (float)int16, real the float itself.  A sample is clipped when
+ * a component is full scale: u8 0 or 255, CS16 -32768 or 32767, real x <= -1 or x >= 2047/2048 (the end codes of a 12-bit
+ * converter scaled (code - 2048)/2048).  The full-scale amplitude fs is 127.5 (u8), 32768 (CS16), 1.0 (real): the mean
+ * power in dBFS is 10*log10(power_sum / samples / fs^2).  Ragged submits count each stream's own rows only; envelope
+ * input (acb_submit_dm_host) leaves this table untouched. */
+typedef struct {
+	uint64_t samples;      /* input samples of the rows produced: rows * K (complex for u8 / CS16, real for real input) */
+	uint64_t clipped;      /* samples with a full-scale component */
+	double   power_sum;    /* sum over those samples of I^2 + Q^2 (real: x^2), converted as above */
+	float    peak;         /* largest |component| of a converted sample (0 before any) */
+	float    pad;
+} acb_input_level_t;
+/* Envelope, per chain, in the envelope's own units (the reference's scale).  Windows are the rows [1024*j, 1024*(j+1))
+ * counted from the stream's own start (acb_create, acb_reset, acb_reset_stream); a window may span submits and counts for
+ * the submit that completes it. */
+typedef struct {
+	uint64_t rows;         /* envelope samples */
+	double   power_sum;    /* sum of dm^2 */
+	float    peak;         /* largest dm (0 before any) */
+	float    pad;
+	uint64_t windows;      /* windows of 1024 rows completed */
+	double   floor;        /* smallest window mean of dm^2 among them; 0 when windows == 0 */
+} acb_chan_level_t;
+/* Fills in[s] (n_in >= nstreams) and ch[s*nch + c] (n_ch >= nstreams*nch); either may be NULL.  The tables cover exactly
+ * the submits acb_collect / acb_sync have covered; reset != 0 clears them after reading (an open window's partial sum is
+ * kept, so the window alignment stays); acb_reset clears everything; acb_reset_stream clears that stream's rows and open
+ * window, queued behind the work in flight, and no other stream's.  ACB_ERR_ARG without ACB_FLAG_LEVEL_STATS. */
+int acb_get_level_stats(acb_ctx_t *ctx, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset);
+
 /* ---- one process, several GPUs (the C host's way to a whole node; SURVEY.md §8e) ----
  *
  * acb_multi_* fronts one context per device.  Two ways to cut the work, neither with any device-to-device
@@ -569,6 +610,9 @@ int  acb_multi_get_state(acb_multi_t *m, int stream, int chn, acb_chan_state_t *
 int  acb_multi_set_state(acb_multi_t *m, int stream, int chn, const acb_chan_state_t *in);
 /* acb_get_decode_stats over the parts, indexed by global stream and channel: out[s*nch + c], n >= nstreams*nch */
 int  acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *out, size_t n, int reset);
+/* acb_get_level_stats over the parts, indexed globally.  A stream split takes each part's streams.  In a channel split
+ * every part reads the same samples, so in[] comes from part 0; ch[] from each part's channels. */
+int  acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset);
 
 /* Block FEC on one frame in place on the HOST (acars.c:123-207): 1 = deliver, 0 = drop.  The
  * processing path runs the same repair on the device (k_block_fec, one thread per frame, right

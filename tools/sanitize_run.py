@@ -130,4 +130,29 @@ for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
             else:
                 ctx.submit_tensor(dev, counts=counts)
         ctx.sync()
+# ACB_FLAG_LEVEL_STATS: k_level_in on each input kind (a ragged u8 device submit, a CS16 length that is no whole number
+# of 16-byte loads), k_level_dm on the channelizer's envelope and on envelope input
+with api.Context(K, 3, 3, 2, flags=1 | api.FLAG_LEVEL_STATS, taps=2 * K + 3) as ctx:
+    for s in range(3):
+        ctx.set_plan(s, fd[:3])
+    bb = 1024 * K * 2
+    dev = torch.randint(0, 256, (3, 2 * bb), dtype=torch.uint8, device="cuda")
+    ctx.submit_device(dev.data_ptr(), 0, 2 * bb, counts=[2, 0, 1])
+    ctx.submit_dm(np.ones((3, 1500, 3), np.float32))
+    ctx.sync()
+    ctx.level_stats()
+for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
+    with api.Context(Kd, 3, 3, 1, flags=fl | api.FLAG_LEVEL_STATS) as ctx:
+        for s in range(3):
+            ctx.set_plan_air(s, fda) if kind == "real" else ctx.set_plan_cs16(s, fd[:3], 0)
+        n = 3 * Kd + 7
+        dev = (torch.randn((3, n), device="cuda") * 0.5 if kind == "real"
+               else torch.randint(-32768, 32767, (3, n, 2), dtype=torch.int16, device="cuda"))
+        if kind == "planar":
+            planes = dev.permute(2, 0, 1).contiguous()
+            ctx.submit_tensor(planes[0], planes[1], counts=[n, 5, Kd + 1])
+        else:
+            ctx.submit_tensor(dev, counts=[n, 5, Kd + 1])
+        ctx.sync()
+        ctx.level_stats()
 print("sanitize run ok", n1, n3, n4, n5)
