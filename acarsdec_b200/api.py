@@ -104,6 +104,12 @@ CHAN_LEVEL_DTYPE = np.dtype([("rows", "<u8"), ("power_sum", "<f8"), ("peak", "<f
 FULL_SCALE = {"u8": 127.5, "cs16": 32768.0, "real": 1.0}
 
 
+class BlobInfo(C.Structure):
+    """acb_streams_blob_info_t: the fingerprint of a stream blob (Context.save_streams)."""
+    _fields_ = [("in_kind", C.c_int), ("K", C.c_int), ("taps", C.c_int), ("nch", C.c_int), ("form", C.c_int), ("flags", C.c_int),
+                ("group_unit", C.c_int), ("group_period", C.c_uint64), ("count", C.c_int), ("record_bytes", C.c_uint64)]
+
+
 # every symbol include/acars_b200.h declares: (name, restype, argtypes)
 ABI = [
     ("acb_round_freq", C.c_int, [C.c_double]),
@@ -202,6 +208,13 @@ ABI = [
     ("acb_multi_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_multi_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_streams_blob_bytes", C.c_size_t, [C.c_void_p, C.c_int]),
+    ("acb_save_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    ("acb_load_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    ("acb_streams_blob_check", C.c_int, [C.c_void_p, C.c_size_t, C.POINTER(BlobInfo)]),
+    ("acb_multi_streams_blob_bytes", C.c_size_t, [C.c_void_p, C.c_int]),
+    ("acb_multi_save_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
+    ("acb_multi_load_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
     ("acb_block_fec", C.c_int, [C.POINTER(Msg)]),
     ("acb_block_fec_batch", C.c_int, [C.c_void_p, C.POINTER(Msg), C.c_int, C.POINTER(C.c_int)]),
     ("acb_crc_update", C.c_uint16, [C.c_uint16, C.c_uint8]),
@@ -279,6 +292,30 @@ def fast_plan(K: int, freqs_hz, fc: int):
     if lib.acb_fast_plan(f.ctypes.data, len(f), K, fc, k.ctypes.data, tw.ctypes.data) != 1:
         return None
     return k, tw[..., 0] + 1j * tw[..., 1]
+
+
+def blob_info(blob: bytes) -> BlobInfo:
+    """acb_streams_blob_check: the fingerprint of a stream blob; AcbError when it is not a valid one (magic, version,
+    size, CRC).  Host only."""
+    lib = load()
+    info = BlobInfo()
+    _check(lib, lib.acb_streams_blob_check(blob, len(blob), C.byref(info)))
+    return info
+
+
+def _save_streams(lib, bytes_fn, save_fn, h, streams) -> bytes:
+    s = np.ascontiguousarray(streams, dtype=np.int32).reshape(-1)
+    n = bytes_fn(h, len(s))
+    if n == 0:
+        raise AcbError("no stream blob for this context / stream count")
+    buf = C.create_string_buffer(n)
+    _check(lib, save_fn(h, s.ctypes.data, len(s), buf, n))
+    return buf.raw
+
+
+def _load_streams(lib, load_fn, h, streams, blob: bytes) -> None:
+    s = np.ascontiguousarray(streams, dtype=np.int32).reshape(-1)
+    _check(lib, load_fn(h, s.ctypes.data, len(s), bytes(blob), len(blob)))
 
 
 def msg_fields(m: Msg) -> Fields | None:
@@ -746,6 +783,15 @@ class Context:
         another stream (torch.cuda.Event.cuda_event)."""
         _check(self.lib, self.lib.acb_wait_event(self.h, cuda_event))
 
+    def save_streams(self, streams) -> bytes:
+        """acb_save_streams: the whole decoding state of these streams (record i = streams[i]) after every submit made so
+        far; the submits in flight are collected first, the context is otherwise unchanged."""
+        return _save_streams(self.lib, self.lib.acb_streams_blob_bytes, self.lib.acb_save_streams, self.h, streams)
+
+    def load_streams(self, streams, blob: bytes) -> None:
+        """acb_load_streams: record i of blob into stream streams[i], queued behind the work in flight."""
+        _load_streams(self.lib, self.lib.acb_load_streams, self.h, streams, blob)
+
 
 class MultiContext:
     """acb_multi_t: one process, several GPUs; streams (mode 0) or channels (mode 1) split among them."""
@@ -904,3 +950,11 @@ class MultiContext:
         s = ChanState()
         _check(self.lib, self.lib.acb_multi_get_state(self.h, stream, chn, C.byref(s)))
         return s
+
+    def save_streams(self, streams) -> bytes:
+        """acb_multi_save_streams (stream split): the blob a single context would give."""
+        return _save_streams(self.lib, self.lib.acb_multi_streams_blob_bytes, self.lib.acb_multi_save_streams, self.h, streams)
+
+    def load_streams(self, streams, blob: bytes) -> None:
+        """acb_multi_load_streams (stream split): collects the submits in flight, then loads each record on its part."""
+        _load_streams(self.lib, self.lib.acb_multi_load_streams, self.h, streams, blob)

@@ -17,7 +17,7 @@ constexpr int TXTCAP = 256;     /* >= acarsdec.h:55's 250, padded */
 
 /* Persistent per-(stream,channel) demodulator + framing state in HBM: what channel_t carries
  * between demodMSK calls (acarsdec.h:76-89; msk.c:71-72,134-135), plus the frame being
- * assembled (msgblk_t, acarsdec.h:48-57).  8-byte aligned, 448 bytes. */
+ * assembled (msgblk_t, acarsdec.h:48-57).  8-byte aligned, 432 bytes. */
 struct ChainState {
 	double phi, df, lvlsum;           /* MskPhi, MskDf, MskLvlSum */
 	float clk;                        /* MskClk (float state!) */
@@ -88,6 +88,7 @@ extern "C" int acb_wb_twiddles(int variant, int K, float *E);
 
 /* kernels.cu entry points (host-callable launchers) */
 struct CUstream_st;
+struct acb_ctx;
 namespace acb {
 enum InputKind { IN_KIND_U8IQ = 0, IN_KIND_F32REAL = 1, IN_KIND_CS16IQ = 2 };
 /* Input history of a context with taps > K (the overlapping window): stream s's last `hpad` samples before the submit
@@ -172,10 +173,47 @@ int launch_level_input(int in_kind, const uint8_t *in, size_t stride, int K, int
                        LevelPart *part, size_t part_stride, LevelIn *out, CUstream_st *stream, int &launched);
 int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int nstreams, double *seg_sum, float *seg_peak,
                     int seg_stride, LevelCarry *carry, LevelChan *out, CUstream_st *stream, int &launched);
+/* Moving streams: each stream's device state is up to SP_MAXREG regions, stream s's `bytes` (a multiple of 4) at
+ * base + s*stride, placed at `off` (a multiple of 16) in its record.  launch_stream_move copies list[i]'s regions to
+ * (unpack = false: k_stream_pack) or from (true: k_stream_unpack) record i at rec + i*rec_bytes, in one launch; it fills
+ * chunk0 itself, adds the kernel to `launched` and returns a cudaError_t. */
+constexpr int SP_MAXREG = 8;
+struct StreamRegion { uint8_t *base; size_t stride, bytes, off; };
+struct StreamRegions { StreamRegion r[SP_MAXREG]; unsigned chunk0[SP_MAXREG + 1]; int nreg; };
+int launch_stream_move(StreamRegions R, const int *list, int n, uint8_t *rec, size_t rec_bytes, bool unpack, CUstream_st *stream,
+                       int &launched);
 int upload_matched_filter(const float *h, CUstream_st *stream);
 int upload_sincos_table(const double *cos_hi_lo, const double *sin_hi_lo, CUstream_st *stream);
 
 /* context.cu, host side, shared with multi.cpp */
+/* stream blobs (acb_save_streams): the header's size; mv_seal sets a blob's record count and CRC; mv_validate is every
+ * refusal of acb_load_streams(c, ..., n, blob, size) that does not depend on the stream list */
+constexpr size_t MV_HEAD_BYTES = 64;
+void mv_seal(void *blob, size_t size, int count);
+int mv_validate(::acb_ctx *c, const void *blob, size_t size, int n);
+struct MvHead {
+	char magic[8];
+	uint32_t version, crc;
+	int32_t in_kind, K, taps, nch, form, flags, group_unit, count;
+	uint64_t group_period, record_bytes;
+};
+static_assert(sizeof(MvHead) == 64, "the blob header is 64 bytes");
+struct MvRecHead { uint64_t pos, carry; uint32_t fast_ok, pad; uint64_t pad2; };
+static_assert(sizeof(MvRecHead) == 32, "the record's host part is 32 bytes");
+constexpr int MV_FLAGS = 256 | 512;            /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS */
+enum MvRegion { R_STATE, R_IN, R_WF, R_TW, R_TWMETA, R_WBMETA, R_LCARRY };
+/* A record of a configuration: its device regions (tag, offset, bytes) in order, then the statistics' offsets */
+struct MvLayout {
+	int nreg;
+	int tag[SP_MAXREG];
+	size_t off[SP_MAXREG], bytes[SP_MAXREG];
+	size_t off_dstats, off_lin, off_lch, rec_bytes;
+};
+MvLayout mv_layout(int in_kind, int K, int taps, int nch, int form, int flags);
+/* a blob header of this context's configuration: magic, version and fingerprint (count and CRC left 0) */
+void mv_fingerprint(::acb_ctx *c, MvHead &h);
+/* the wideband plan of one stream (nct = ceil(nch / WB_CTILE) blocks of WB_META ints) from its channels' bins */
+void wb_meta(int in_kind, int nch, const int *kbin, int etab, int *meta);
 /* sets the message acb_last_error() returns (of the calling thread); returns `code` */
 int fail(int code, const char *fmt, ...);
 /* Emission-group starts of a streaming submit that covers envelope samples [pos, pos + nout): the first is pos, then

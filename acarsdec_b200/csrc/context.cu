@@ -200,6 +200,12 @@ struct acb_ctx {
 	cudaEvent_t ev_rag_used[NRAG][3];             /* behind the last reads of slot i on the copy, channelizer and demod streams */
 	bool rag_used[NRAG];
 	unsigned long long rag_seq;
+	/* acb_save_streams / acb_load_streams: [stream list | records] staging, grown on demand; ev_mv follows the last load's
+	 * unpack, which reads d_mv */
+	uint8_t *d_mv, *h_mv;                         /* h_mv pinned */
+	size_t mv_cap;
+	cudaEvent_t ev_mv;
+	bool mv_pending;
 };
 
 static void consumer_main(acb_ctx *c);
@@ -303,6 +309,26 @@ static int reset_states(acb_ctx *c)
 	return ACB_OK;
 }
 
+/* The history (hpad samples) and padded table length (taps_pad) of a context of this kind, K, taps and form */
+static void taps_geometry(int in_kind, int K, int taps, ChanForm form, int &hpad, int &taps_pad)
+{
+	const int per_unit = in_kind != IN_KIND_U8IQ ? 4 : 8;   /* taps per 16 bytes of input (4-byte vs 2-byte taps) */
+	hpad = 0;
+	if (taps > K) {
+		/* overlapping window: H = taps - K samples of the previous rows, rounded up to whole units and padded in
+		 * FRONT with zero weights (acb_set_wf).  Leading zero-weight terms leave the sum unchanged: the accumulator
+		 * starts at +0, each such term is a product with a zero weight, i.e. +-0 (finite input), and +0 + (+-0) = +0
+		 * in round-to-nearest, so the accumulator is still exactly +0 when the first real term p arrives, and
+		 * +0 + p = p is what the unpadded sum starts with.  That holds for any K, so the generic kernel uses the same
+		 * layout. */
+		hpad = (taps - K + per_unit - 1) / per_unit * per_unit;
+		taps_pad = K + hpad;
+	} else {
+		taps_pad = form == CHAN_GENERIC ? taps : (taps + per_unit - 1) / per_unit * per_unit;
+		if (taps_pad > K) taps_pad = K;      /* K itself is a multiple of per_unit here */
+	}
+}
+
 extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 {
 	if (!cfg || !out) return fail(ACB_ERR_ARG, "null argument");
@@ -331,23 +357,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->real_input = c->in_kind != IN_KIND_U8IQ;
 	c->taps = cfg->taps ? cfg->taps : cfg->K;
 	c->form = chan_form(c->in_kind, cfg->K, c->taps, cfg->flags);
-	{
-		const int per_unit = c->real_input ? 4 : 8;          /* taps per 16 bytes of input (4-byte vs 2-byte taps) */
-		c->hpad = 0;
-		if (c->taps > cfg->K) {
-			/* overlapping window: H = taps - K samples of the previous rows, rounded up to whole units and padded in
-			 * FRONT with zero weights (acb_set_wf).  Leading zero-weight terms leave the sum unchanged: the accumulator
-			 * starts at +0, each such term is a product with a zero weight, i.e. +-0 (finite input), and +0 + (+-0) = +0
-			 * in round-to-nearest, so the accumulator is still exactly +0 when the first real term p arrives, and
-			 * +0 + p = p is what the unpadded sum starts with.  That holds for any K, so the generic kernel uses the same
-			 * layout. */
-			c->hpad = (c->taps - cfg->K + per_unit - 1) / per_unit * per_unit;
-			c->taps_pad = cfg->K + c->hpad;
-		} else {
-			c->taps_pad = c->form == CHAN_GENERIC ? c->taps : (c->taps + per_unit - 1) / per_unit * per_unit;
-			if (c->taps_pad > cfg->K) c->taps_pad = cfg->K;      /* K itself is a multiple of per_unit here */
-		}
-	}
+	taps_geometry(c->in_kind, cfg->K, c->taps, c->form, c->hpad, c->taps_pad);
 	c->d_hist = nullptr;
 	c->d_real[0] = c->d_real[1] = nullptr;
 	c->d_planar = nullptr;
@@ -380,6 +390,10 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->d_lseg_sum = nullptr;
 	c->d_lseg_peak = nullptr;
 	c->d_lcarry = nullptr;
+	c->d_mv = c->h_mv = nullptr;
+	c->mv_cap = 0;
+	c->ev_mv = nullptr;
+	c->mv_pending = false;
 	*out = c;
 
 	{
@@ -397,6 +411,7 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaStreamCreateWithPriority(&c->s_d2h, cudaStreamNonBlocking, greatest));
 	}
 	CU(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
+	CU(cudaEventCreateWithFlags(&c->ev_mv, cudaEventDisableTiming));
 	CU(cudaEventCreate(&c->mark[0]));
 	CU(cudaEventCreate(&c->mark[1]));
 	const size_t in_bytes = (size_t)cfg->nstreams * cfg->max_blocks * c->blk_bytes;
@@ -594,6 +609,8 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 			if (c->ev_lvl_done[i]) cudaEventDestroy(c->ev_lvl_done[i]);
 		}
 		cudaFree(c->d_lpart); cudaFree(c->d_lseg_sum); cudaFree(c->d_lseg_peak); cudaFree(c->d_lcarry);
+		cudaFree(c->d_mv); cudaFreeHost(c->h_mv);
+		if (c->ev_mv) cudaEventDestroy(c->ev_mv);
 		for (int i = 0; i < NRAG; i++) {
 			if (!c->d_rag[i]) continue;
 			cudaFree(c->d_rag[i]); cudaFreeHost(c->h_rag[i]);
@@ -699,12 +716,12 @@ static int upload_fast_plan(acb_ctx *c, int stream, const std::vector<int> &kbin
 /* wideband form: per channel tile, the channel slots sorted by bin residue (k/2) mod 4 (real input: by the column the
  * real form reads, k mod 4 = 0, 2 or odd) and each class padded to whole groups of WB_CB (channel -1), so that every
  * thread of k_channelize_wb(_real) multiplies one Y' column; `etab` selects the twiddle table (CS16: the variant) */
-static int upload_wb_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, int etab)
+void acb::wb_meta(int in_kind, int nch, const int *kbin, int etab, int *meta)
 {
-	const int nch = c->cfg.nch, nct = (nch + WB_CTILE - 1) / WB_CTILE;
-	const bool real = c->in_kind == IN_KIND_F32REAL;
+	const int nct = (nch + WB_CTILE - 1) / WB_CTILE;
+	const bool real = in_kind == IN_KIND_F32REAL;
 	auto cls = [real](int k) { return real ? ((k & 3) == 0 ? 0 : (k & 3) == 2 ? 1 : 2) : (((k / 2) % 4) + 4) % 4; };
-	std::vector<int> meta((size_t)nct * WB_META, 0);
+	std::fill(meta, meta + (size_t)nct * WB_META, 0);
 	for (int z = 0; z < nct; z++) {
 		int *m = &meta[(size_t)z * WB_META];
 		int slot = 0;
@@ -723,6 +740,13 @@ static int upload_wb_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, 
 		m[0] = slot / WB_CB;
 		m[1] = etab;
 	}
+}
+
+static int upload_wb_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, int etab)
+{
+	const int nct = (c->cfg.nch + WB_CTILE - 1) / WB_CTILE;
+	std::vector<int> meta((size_t)nct * WB_META);
+	wb_meta(c->in_kind, c->cfg.nch, kbin.data(), etab, meta.data());
 	if (int r = upload(c, c->d_wbmeta + (size_t)stream * meta.size(), meta.data(), meta.size() * sizeof(int))) return r;
 	c->fast_ok[stream] = 1;
 	return ACB_OK;
@@ -2003,6 +2027,363 @@ extern "C" int acb_get_level_stats(acb_ctx_t *c, acb_input_level_t *in, size_t n
 	if (reset) {                 /* the open windows stay on the device: the alignment is kept */
 		memset(c->lin.data(), 0, c->lin.size() * sizeof(acb_input_level_t));
 		memset(c->lch.data(), 0, c->lch.size() * sizeof(acb_chan_level_t));
+	}
+	return ACB_OK;
+}
+
+/* ---- moving streams (acb_save_streams / acb_load_streams) ----
+ *
+ * Blob: a 64-byte header (MvHead), then `count` records of record_bytes each.  A record is a 32-byte host part (MvRecHead),
+ * the device regions of mv_layout at 16-byte aligned offsets (copied verbatim by k_stream_pack / k_stream_unpack), then
+ * the host statistics: nch acb_decode_stats_t (ACB_FLAG_DECODE_STATS), one acb_input_level_t and nch acb_chan_level_t
+ * (ACB_FLAG_LEVEL_STATS).  The CRC-32 (IEEE, as zlib's crc32) covers every byte from offset 16 to the end. */
+namespace {
+constexpr char MV_MAGIC[8] = { 'A', 'C', 'B', 'S', 'T', 'R', 'M', 0 };
+/* The records copy these layouts verbatim, so a blob of one version means them: change any of them (a field moved, a
+ * size, a table's order) and MV_VERSION must change with it, or old blobs would load without error and decode wrong.
+ * The asserts pin what the version stands for today. */
+constexpr uint32_t MV_VERSION = 1;
+static_assert(sizeof(ChainState) == 432 && offsetof(ChainState, state) == 44 && offsetof(ChainState, pos) == 64 &&
+              offsetof(ChainState, inb_re) == 80 && offsetof(ChainState, crc) == 168 && offsetof(ChainState, txt) == 176,
+              "ChainState changed: bump MV_VERSION");
+static_assert(sizeof(LevelCarry) == 16 && offsetof(LevelCarry, rows) == 8, "LevelCarry changed: bump MV_VERSION");
+static_assert(CH_GROUP == 8 && WB_CTILE == 256 && WB_CB == 4 && WB_META == 546, "table layouts changed: bump MV_VERSION");
+static_assert(sizeof(acb_decode_stats_t) == 120 && sizeof(acb_input_level_t) == 32 && sizeof(acb_chan_level_t) == 40,
+              "statistics changed: bump MV_VERSION");
+}
+
+static size_t round16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+/* The record of a configuration; the same for every context of it, whatever its nstreams, max_blocks or device */
+MvLayout acb::mv_layout(int in_kind, int K, int taps, int nch, int form, int flags)
+{
+	MvLayout L{};
+	int hpad = 0, taps_pad = 0;
+	taps_geometry(in_kind, K, taps, (ChanForm)form, hpad, taps_pad);
+	const size_t ngrp = (size_t)(nch + CH_GROUP - 1) / CH_GROUP, nct = (size_t)(nch + WB_CTILE - 1) / WB_CTILE;
+	size_t off = sizeof(MvRecHead);
+	auto add = [&](int tag, size_t bytes) {
+		L.tag[L.nreg] = tag;
+		L.off[L.nreg] = off;
+		L.bytes[L.nreg] = bytes;
+		L.nreg++;
+		off += round16(bytes);
+	};
+	add(R_STATE, (size_t)nch * sizeof(ChainState));
+	if (in_kind != IN_KIND_U8IQ) add(R_IN, round16(((size_t)hpad + K) * 4));     /* history + carry (< K samples) */
+	else if (hpad) add(R_IN, (size_t)hpad * 2);
+	add(R_WF, ngrp * taps_pad * CH_GROUP * 2 * sizeof(float));
+	if (form == CHAN_DFT || form == CHAN_RDFT || form == CHAN_OVL_FAST || form == CHAN_OVL_RDFT) {
+		add(R_TW, ngrp * CH_GROUP * (K / 4) * 2 * sizeof(float));
+		add(R_TWMETA, ngrp * sizeof(unsigned));
+	}
+	if (form == CHAN_WB || form == CHAN_WB_REAL) add(R_WBMETA, nct * WB_META * sizeof(int));
+	if (flags & ACB_FLAG_LEVEL_STATS) add(R_LCARRY, (size_t)nch * sizeof(LevelCarry));
+	L.off_dstats = off;
+	if (flags & ACB_FLAG_DECODE_STATS) off += (size_t)nch * sizeof(acb_decode_stats_t);
+	L.off_lin = off;
+	L.off_lch = off + sizeof(acb_input_level_t);
+	if (flags & ACB_FLAG_LEVEL_STATS) off += sizeof(acb_input_level_t) + (size_t)nch * sizeof(acb_chan_level_t);
+	L.rec_bytes = round16(off);
+	return L;
+}
+
+static MvLayout ctx_layout(const acb_ctx *c)
+{
+	return mv_layout(c->in_kind, c->cfg.K, c->taps, c->cfg.nch, c->form, c->cfg.flags & MV_FLAGS);
+}
+
+/* CRC-32 (IEEE, as zlib's crc32), eight bytes per step (slicing-by-8): moving a whole context is host-bound, and this
+ * runs over every byte of a blob on save and on load */
+static uint32_t crc32_update(uint32_t crc, const uint8_t *p, size_t n)
+{
+	struct Tables {
+		uint32_t t[8][256];
+		Tables()
+		{
+			for (uint32_t i = 0; i < 256; i++) {
+				uint32_t v = i;
+				for (int k = 0; k < 8; k++) v = v & 1 ? 0xEDB88320u ^ (v >> 1) : v >> 1;
+				t[0][i] = v;
+			}
+			for (int k = 1; k < 8; k++)
+				for (int i = 0; i < 256; i++) t[k][i] = (t[k - 1][i] >> 8) ^ t[0][t[k - 1][i] & 0xff];
+		}
+	};
+	static const Tables T;                       /* initialised once, thread-safely */
+	crc = ~crc;
+	for (; n >= 8; n -= 8, p += 8) {
+		uint32_t a, b;
+		memcpy(&a, p, 4);                        /* the blob is little-endian, as the host is */
+		memcpy(&b, p + 4, 4);
+		a ^= crc;
+		crc = T.t[7][a & 0xff] ^ T.t[6][(a >> 8) & 0xff] ^ T.t[5][(a >> 16) & 0xff] ^ T.t[4][a >> 24] ^ T.t[3][b & 0xff] ^
+		      T.t[2][(b >> 8) & 0xff] ^ T.t[1][(b >> 16) & 0xff] ^ T.t[0][b >> 24];
+	}
+	for (; n; n--, p++) crc = T.t[0][(crc ^ *p) & 0xff] ^ (crc >> 8);
+	return ~crc;
+}
+
+void acb::mv_seal(void *blob, size_t size, int count)
+{
+	MvHead h;
+	memcpy(&h, blob, sizeof(h));
+	h.count = count;
+	memcpy(blob, &h, sizeof(h));
+	const uint32_t crc = crc32_update(0, (const uint8_t *)blob + 16, size - 16);
+	memcpy((uint8_t *)blob + offsetof(MvHead, crc), &crc, 4);
+}
+
+extern "C" int acb_streams_blob_check(const void *blob, size_t size, acb_streams_blob_info_t *out)
+{
+	if (!blob) return fail(ACB_ERR_ARG, "null blob");
+	if (size < sizeof(MvHead)) return fail(ACB_ERR_ARG, "blob of %zu bytes is shorter than its header", size);
+	MvHead h;
+	memcpy(&h, blob, sizeof(h));
+	if (memcmp(h.magic, MV_MAGIC, sizeof(MV_MAGIC))) return fail(ACB_ERR_ARG, "not a stream blob (magic)");
+	if (h.version != MV_VERSION) return fail(ACB_ERR_ARG, "blob format version %u, this library reads %u", h.version, MV_VERSION);
+	if (h.in_kind < IN_KIND_U8IQ || h.in_kind > IN_KIND_CS16IQ || h.K < 1 || h.K > ACB_MAXK || h.taps < 1 ||
+	    h.taps > ACB_MAXTAPS_PER_K * h.K || h.nch < 1 || h.form < CHAN_EXACT || h.form > CHAN_WB_REAL || (h.flags & ~MV_FLAGS) ||
+	    h.count < 1)
+		return fail(ACB_ERR_ARG, "blob header out of range");
+	const MvLayout L = mv_layout(h.in_kind, h.K, h.taps, h.nch, h.form, h.flags);
+	if (h.record_bytes != L.rec_bytes) return fail(ACB_ERR_ARG, "blob records of %llu bytes, the configuration's are %zu",
+	                                               (unsigned long long)h.record_bytes, L.rec_bytes);
+	if ((size - sizeof(MvHead)) / L.rec_bytes != (size_t)h.count || (size - sizeof(MvHead)) % L.rec_bytes)
+		return fail(ACB_ERR_ARG, "blob of %zu bytes does not hold %d records of %zu bytes", size, h.count, L.rec_bytes);
+	if (crc32_update(0, (const uint8_t *)blob + 16, size - 16) != h.crc) return fail(ACB_ERR_ARG, "blob CRC mismatch");
+	if (out) {
+		out->in_kind = h.in_kind; out->K = h.K; out->taps = h.taps; out->nch = h.nch; out->form = h.form; out->flags = h.flags;
+		out->group_unit = h.group_unit; out->group_period = h.group_period; out->count = h.count; out->record_bytes = h.record_bytes;
+	}
+	return ACB_OK;
+}
+
+extern "C" size_t acb_streams_blob_bytes(acb_ctx_t *c, int n)
+{
+	if (!c || n < 1) return 0;
+	return sizeof(MvHead) + (size_t)n * ctx_layout(c).rec_bytes;
+}
+
+/* n distinct streams in range */
+static int mv_check_list(const acb_ctx *c, const int *streams, int n)
+{
+	if (n < 1 || n > c->cfg.nstreams) return fail(ACB_ERR_ARG, "n=%d outside 1..nstreams=%d", n, c->cfg.nstreams);
+	std::vector<unsigned char> seen(c->cfg.nstreams, 0);
+	for (int i = 0; i < n; i++) {
+		if (streams[i] < 0 || streams[i] >= c->cfg.nstreams) return fail(ACB_ERR_ARG, "stream %d out of range", streams[i]);
+		if (seen[streams[i]]++) return fail(ACB_ERR_ARG, "stream %d listed twice", streams[i]);
+	}
+	return ACB_OK;
+}
+
+/* room for the list and n records in both stagings, once the last load's unpack has read the device one */
+static int mv_stage(acb_ctx *c, size_t bytes)
+{
+	if (c->mv_pending) {
+		CU(cudaEventSynchronize(c->ev_mv));
+		c->mv_pending = false;
+	}
+	if (bytes <= c->mv_cap) return ACB_OK;
+	cudaFree(c->d_mv);
+	cudaFreeHost(c->h_mv);
+	c->d_mv = c->h_mv = nullptr;
+	c->mv_cap = 0;
+	CU(cudaMalloc(&c->d_mv, bytes));
+	CU(cudaHostAlloc(&c->h_mv, bytes, cudaHostAllocDefault));
+	c->mv_cap = bytes;
+	return ACB_OK;
+}
+
+/* where each region of L lives in this context */
+static StreamRegions mv_regions(const acb_ctx *c, const MvLayout &L)
+{
+	StreamRegions R{};
+	R.nreg = L.nreg;
+	for (int k = 0; k < L.nreg; k++) {
+		StreamRegion &g = R.r[k];
+		g.bytes = L.bytes[k];
+		g.off = L.off[k];
+		g.stride = L.bytes[k];
+		switch (L.tag[k]) {
+		case R_STATE: g.base = (uint8_t *)c->d_state; break;
+		case R_IN:
+			if (c->real_input) {
+				g.base = (uint8_t *)c->d_real[c->real_buf];     /* [history | carry] in front of the next submit's samples */
+				g.stride = c->real_cap * sizeof(float);
+			} else {
+				g.base = c->d_hist;
+			}
+			break;
+		case R_WF: g.base = (uint8_t *)c->d_wf; break;
+		case R_TW: g.base = (uint8_t *)c->d_tw; break;
+		case R_TWMETA: g.base = (uint8_t *)c->d_twmeta; break;
+		case R_WBMETA: g.base = (uint8_t *)c->d_wbmeta; break;
+		case R_LCARRY: g.base = (uint8_t *)c->d_lcarry; break;
+		}
+	}
+	return R;
+}
+
+void acb::mv_fingerprint(acb_ctx_t *c, MvHead &h)
+{
+	h = MvHead{};
+	memcpy(h.magic, MV_MAGIC, sizeof(MV_MAGIC));
+	h.version = MV_VERSION;
+	h.in_kind = c->in_kind; h.K = c->cfg.K; h.taps = c->taps; h.nch = c->cfg.nch; h.form = c->form; h.flags = c->cfg.flags & MV_FLAGS;
+	h.group_unit = c->real_input ? c->group_unit : 0;
+	h.group_period = c->real_input ? c->group_period : 0;
+	h.record_bytes = ctx_layout(c).rec_bytes;
+}
+
+extern "C" int acb_save_streams(acb_ctx_t *c, const int *streams, int n, void *blob, size_t cap)
+{
+	if (!c || !streams || !blob) return fail(ACB_ERR_ARG, "null argument");
+	if (int r = mv_check_list(c, streams, n)) return r;
+	const MvLayout L = ctx_layout(c);
+	const size_t rec = L.rec_bytes, need = sizeof(MvHead) + (size_t)n * rec, lb = round16((size_t)n * sizeof(int));
+	if (cap < need) return fail(ACB_ERR_ARG, "cap=%zu < %zu bytes", cap, need);
+	if (int r = ctx_use(c)) return r;
+	/* every submit made so far, as acb_sync collects them (an overflow stays for acb_collect / acb_sync to report) */
+	while (!c->inflight.empty())
+		if (int r = collect_oldest(c)) return r;
+	if (int r = sync_streams(c)) return r;
+	wait_consumer(c, c->jobs_queued);
+	if (c->consumer_err[0]) return fail(ACB_ERR_CUDA, "%s", c->consumer_err);
+	if (int r = mv_stage(c, lb + (size_t)n * rec)) return r;
+	memcpy(c->h_mv, streams, (size_t)n * sizeof(int));
+	CU(cudaMemcpyAsync(c->d_mv, c->h_mv, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, c->s_comp));
+	int launched = 0;
+	if (int r = launch_stream_move(mv_regions(c, L), (const int *)c->d_mv, n, c->d_mv + lb, rec, false, c->s_comp, launched))
+		return fail(ACB_ERR_CUDA, "stream pack launch: %s", cudaGetErrorString((cudaError_t)r));
+	c->stats.kernel_launches += launched;
+	CU(cudaMemcpyAsync(c->h_mv + lb, c->d_mv + lb, (size_t)n * rec, cudaMemcpyDeviceToHost, c->s_comp));
+	CU(cudaStreamSynchronize(c->s_comp));
+	uint8_t *const out = (uint8_t *)blob;
+	MvHead h;
+	mv_fingerprint(c, h);
+	memcpy(out, &h, sizeof(h));
+	memcpy(out + sizeof(MvHead), c->h_mv + lb, (size_t)n * rec);
+	const int nch = c->cfg.nch;
+	for (int i = 0; i < n; i++) {
+		const int s = streams[i];
+		uint8_t *r = out + sizeof(MvHead) + (size_t)i * rec;
+		const MvRecHead rh{ c->pos[s], c->real_input ? (uint64_t)c->carry[s] : 0, c->fast_ok[s], 0, 0 };
+		memcpy(r, &rh, sizeof(rh));
+		for (int k = 0; c->real_input && k < L.nreg; k++) {
+			/* what lies past the history and carry is no state: zeros, so that equal states give equal blobs */
+			const size_t used = ((size_t)c->hpad + c->carry[s]) * sizeof(float);
+			if (L.tag[k] == R_IN) memset(r + L.off[k] + used, 0, L.bytes[k] - used);
+		}
+		if (c->decode_stats) {
+			std::lock_guard<std::mutex> lk(c->dstats_mtx);
+			memcpy(r + L.off_dstats, &c->dstats[(size_t)s * nch], (size_t)nch * sizeof(acb_decode_stats_t));
+		}
+		if (c->level_stats) {
+			std::lock_guard<std::mutex> lk(c->lstats_mtx);
+			memcpy(r + L.off_lin, &c->lin[s], sizeof(acb_input_level_t));
+			memcpy(r + L.off_lch, &c->lch[(size_t)s * nch], (size_t)nch * sizeof(acb_chan_level_t));
+		}
+	}
+	mv_seal(out, need, n);
+	return ACB_OK;
+}
+
+/* Everything acb_load_streams refuses, checked before anything changes: the blob itself, its fingerprint against the
+ * context's, n, and the record fields the device indexes with (a corrupt blob with a valid CRC must not write out of
+ * bounds) */
+int acb::mv_validate(acb_ctx_t *c, const void *blob, size_t size, int n)
+{
+	acb_streams_blob_info_t info;
+	if (int r = acb_streams_blob_check(blob, size, &info)) return r;
+	const int flags = c->cfg.flags & MV_FLAGS;
+	if (info.in_kind != c->in_kind || info.K != c->cfg.K || info.taps != c->taps || info.nch != c->cfg.nch || info.form != c->form)
+		return fail(ACB_ERR_ARG, "blob of kind %d, K=%d, taps=%d, nch=%d, form %d; the context is %d, %d, %d, %d, %d", info.in_kind, info.K,
+		            info.taps, info.nch, info.form, c->in_kind, c->cfg.K, c->taps, c->cfg.nch, (int)c->form);
+	if (info.flags != flags) return fail(ACB_ERR_ARG, "blob statistics flags %d, the context's %d", info.flags, flags);
+	if (c->real_input && (info.group_unit != c->group_unit || info.group_period != c->group_period))
+		return fail(ACB_ERR_ARG, "blob emission groups (%d, %llu) differ from the context's (%d, %llu)", info.group_unit,
+		            (unsigned long long)info.group_period, c->group_unit, (unsigned long long)c->group_period);
+	if (n != info.count) return fail(ACB_ERR_ARG, "n=%d, the blob holds %d records", n, info.count);
+	const MvLayout L = ctx_layout(c);
+	const int nch = c->cfg.nch;
+	for (int i = 0; i < n; i++) {
+		const uint8_t *r = (const uint8_t *)blob + sizeof(MvHead) + (size_t)i * L.rec_bytes;
+		MvRecHead rh;
+		memcpy(&rh, r, sizeof(rh));
+		if (rh.carry >= (uint64_t)(c->real_input ? c->cfg.K : 1) || rh.fast_ok > 1) return fail(ACB_ERR_ARG, "record %d: carry / plan out of range", i);
+		for (int k = 0; k < L.nreg; k++) {
+			if (L.tag[k] == R_STATE) {
+				for (int ch = 0; ch < nch; ch++) {
+					ChainState st;
+					memcpy(&st, r + L.off[k] + (size_t)ch * sizeof(ChainState), sizeof(st));
+					if (st.idx >= (unsigned)FLEN || st.blk_len < 0 || st.blk_len > 248 || st.outbits > 0xffu)
+						return fail(ACB_ERR_ARG, "record %d: chain %d's state out of range", i, ch);
+				}
+			} else if (L.tag[k] == R_WBMETA) {
+				const int ntab = c->in_kind == IN_KIND_CS16IQ ? 2 : 1;
+				for (size_t z = 0; z < L.bytes[k] / (WB_META * sizeof(int)); z++) {
+					int m[WB_META];
+					memcpy(m, r + L.off[k] + z * WB_META * sizeof(int), sizeof(m));
+					bool ok = m[0] >= 0 && m[0] <= WB_SLOTS / WB_CB && m[1] >= 0 && m[1] < ntab;
+					for (int j = 0; ok && j < WB_SLOTS; j++)
+						ok = m[3 + 2 * j] >= -1 && m[3 + 2 * j] < nch && m[2 + 2 * j] > -c->cfg.K && m[2 + 2 * j] < c->cfg.K;
+					if (!ok) return fail(ACB_ERR_ARG, "record %d: wideband plan out of range", i);
+				}
+			}
+		}
+	}
+	return ACB_OK;
+}
+
+extern "C" int acb_load_streams(acb_ctx_t *c, const int *streams, int n, const void *blob, size_t size)
+{
+	if (!c || !streams || !blob) return fail(ACB_ERR_ARG, "null argument");
+	if (int r = mv_check_list(c, streams, n)) return r;
+	if (int r = mv_validate(c, blob, size, n)) return r;
+	if (int r = ctx_use(c)) return r;
+	const MvLayout L = ctx_layout(c);
+	const size_t rec = L.rec_bytes, lb = round16((size_t)n * sizeof(int));
+	const uint8_t *const in = (const uint8_t *)blob + sizeof(MvHead);
+	if (int r = mv_stage(c, lb + (size_t)n * rec)) return r;
+	memcpy(c->h_mv, streams, (size_t)n * sizeof(int));
+	memcpy(c->h_mv + lb, in, (size_t)n * rec);
+	/* as acb_reset_stream: the chain states behind the demods already queued, the input side, tables and open windows
+	 * behind the channelizer, level kernels and tail moves (all on the channelizer stream), and everything ahead of the
+	 * next submit's append and kernels */
+	CU(cudaEventRecord(c->ev_join, c->s_dem));
+	CU(cudaStreamWaitEvent(c->s_comp, c->ev_join, 0));
+	CU(cudaMemcpyAsync(c->d_mv, c->h_mv, lb + (size_t)n * rec, cudaMemcpyHostToDevice, c->s_comp));
+	int launched = 0;
+	if (int r = launch_stream_move(mv_regions(c, L), (const int *)c->d_mv, n, c->d_mv + lb, rec, true, c->s_comp, launched))
+		return fail(ACB_ERR_CUDA, "stream unpack launch: %s", cudaGetErrorString((cudaError_t)r));
+	c->stats.kernel_launches += launched;
+	CU(cudaEventRecord(c->ev_mv, c->s_comp));
+	c->mv_pending = true;
+	CU(cudaEventRecord(c->ev_join, c->s_comp));
+	CU(cudaStreamWaitEvent(c->s_dem, c->ev_join, 0));
+	CU(cudaStreamWaitEvent(c->s_copy, c->ev_join, 0));
+	const int nch = c->cfg.nch;
+	for (int i = 0; i < n; i++) {
+		const int s = streams[i];
+		const uint8_t *r = in + (size_t)i * rec;
+		MvRecHead rh;
+		memcpy(&rh, r, sizeof(rh));
+		c->pos[s] = rh.pos;
+		if (c->real_input) c->carry[s] = (size_t)rh.carry;
+		c->fast_ok[s] = (unsigned char)rh.fast_ok;
+		/* the slot's counts become the blob's; submits made before the load are not counted (acb_reset_stream's rule) */
+		if (c->decode_stats) {
+			std::lock_guard<std::mutex> lk(c->dstats_mtx);
+			memcpy(&c->dstats[(size_t)s * nch], r + L.off_dstats, (size_t)nch * sizeof(acb_decode_stats_t));
+			c->dstats_from[s] = c->nsubmit;
+		}
+		if (c->level_stats) {
+			std::lock_guard<std::mutex> lk(c->lstats_mtx);
+			memcpy(&c->lin[s], r + L.off_lin, sizeof(acb_input_level_t));
+			memcpy(&c->lch[(size_t)s * nch], r + L.off_lch, (size_t)nch * sizeof(acb_chan_level_t));
+			c->lstats_from[s] = c->nsubmit;
+		}
 	}
 	return ACB_OK;
 }

@@ -3875,5 +3875,62 @@ int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int ns
 	return (int)cudaGetLastError();
 }
 
+/* Moving streams (acb_save_streams / acb_load_streams): stream list[i]'s device regions to and from record i of a staging
+ * buffer.  blockIdx.y is the record; blockIdx.x walks the regions in SP_CHUNK pieces (R.chunk0[k] is region k's first).
+ * A piece whose two addresses and ends are all 16-byte aligned moves in 16-byte vectors, any other in 4-byte words (the
+ * fast plans' per-stream metadata has 4-byte strides). */
+constexpr int SP_THREADS = 256;
+constexpr unsigned SP_CHUNK = SP_THREADS * 16 * 4;
+
+template <bool UNPACK>
+__device__ __forceinline__ void stream_copy(const StreamRegions &R, const int *__restrict__ list, uint8_t *rec, size_t rec_bytes)
+{
+	const unsigned x = blockIdx.x;
+	int k = 0;
+	while (k + 1 < R.nreg && x >= R.chunk0[k + 1]) k++;
+	const StreamRegion &g = R.r[k];
+	uint8_t *dev = g.base + (size_t)list[blockIdx.y] * g.stride;
+	uint8_t *blob = rec + (size_t)blockIdx.y * rec_bytes + g.off;
+	const size_t lo = (size_t)(x - R.chunk0[k]) * SP_CHUNK, hi = min(lo + SP_CHUNK, g.bytes);
+	uint8_t *dst = UNPACK ? dev : blob;
+	const uint8_t *src = UNPACK ? blob : dev;
+	if ((((uintptr_t)dev | (uintptr_t)blob | lo | hi) & 15) == 0) {
+		for (size_t b = lo + threadIdx.x * 16; b < hi; b += SP_THREADS * 16)
+			*reinterpret_cast<uint4 *>(dst + b) = *reinterpret_cast<const uint4 *>(src + b);
+	} else {
+		for (size_t b = lo + threadIdx.x * 4; b < hi; b += SP_THREADS * 4)
+			*reinterpret_cast<uint32_t *>(dst + b) = *reinterpret_cast<const uint32_t *>(src + b);
+	}
+}
+
+__global__ void __launch_bounds__(SP_THREADS)
+k_stream_pack(const __grid_constant__ StreamRegions R, const int *__restrict__ list, uint8_t *rec, size_t rec_bytes)
+{
+	stream_copy<false>(R, list, rec, rec_bytes);
+}
+
+__global__ void __launch_bounds__(SP_THREADS)
+k_stream_unpack(const __grid_constant__ StreamRegions R, const int *__restrict__ list, uint8_t *rec, size_t rec_bytes)
+{
+	stream_copy<true>(R, list, rec, rec_bytes);
+}
+
+int launch_stream_move(StreamRegions R, const int *list, int n, uint8_t *rec, size_t rec_bytes, bool unpack, cudaStream_t stream,
+                       int &launched)
+{
+	if (R.nreg < 1 || R.nreg > SP_MAXREG || n < 1 || n > 65535) return (int)cudaErrorInvalidValue;
+	R.chunk0[0] = 0;
+	for (int k = 0; k < R.nreg; k++) {
+		if (R.r[k].bytes % 4 || R.r[k].off % 16 || R.r[k].off + R.r[k].bytes > rec_bytes) return (int)cudaErrorInvalidValue;
+		R.chunk0[k + 1] = R.chunk0[k] + (unsigned)((R.r[k].bytes + SP_CHUNK - 1) / SP_CHUNK);
+	}
+	const dim3 grid(R.chunk0[R.nreg], (unsigned)n);
+	if (grid.x == 0) return 0;
+	if (unpack) k_stream_unpack<<<grid, SP_THREADS, 0, stream>>>(R, list, rec, rec_bytes);
+	else k_stream_pack<<<grid, SP_THREADS, 0, stream>>>(R, list, rec, rec_bytes);
+	launched++;
+	return (int)cudaGetLastError();
+}
+
 } // namespace acb
 

@@ -449,3 +449,257 @@ extern "C" int acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, 
 	}
 	return ACB_OK;
 }
+
+/* ---- moving streams: a blob is the one a single context of cfg gives, whatever the split ----
+ * A stream split saves each stream on the part that owns it (every part has cfg's fingerprint but nstreams).  In a
+ * channel split every part holds every stream but only channels [c0, c0 + nc) of it, in tables laid out for nc channels;
+ * a record is converted between a part's layout and the full one on the host (chan_record), the input side and the input
+ * levels taken from part 0, which reads the same samples as every part. */
+using acb::MvHead;
+using acb::MvLayout;
+using acb::MvRecHead;
+
+static int multi_list(acb_multi *m, const int *streams, int n)
+{
+	if (!streams || n < 1 || n > m->cfg.nstreams) return fail(ACB_ERR_ARG, "n=%d outside 1..nstreams", n);
+	std::vector<unsigned char> seen(m->cfg.nstreams, 0);
+	for (int i = 0; i < n; i++) {
+		if (streams[i] < 0 || streams[i] >= m->cfg.nstreams) return fail(ACB_ERR_ARG, "stream %d out of range", streams[i]);
+		if (seen[streams[i]]++) return fail(ACB_ERR_ARG, "stream %d listed twice", streams[i]);
+	}
+	return ACB_OK;
+}
+
+static size_t part_of(const acb_multi *m, int stream)
+{
+	size_t i = 0;
+	while (stream >= m->parts[i].s0 + m->parts[i].ns) i++;
+	return i;
+}
+
+static MvLayout layout_of(const MvHead &h, int nch)
+{
+	return acb::mv_layout(h.in_kind, h.K, h.taps, nch, h.form, h.flags);
+}
+
+/* Channel split: record `part` (layout P, channels [c0, c0 + nc)) to or from record `full` (layout F, nch channels).
+ * to_full: the part's channels go to their places, part 0 also gives the host part, the input side and the input levels,
+ * and fast_ok is the AND over the parts (the caller starts it at 1), as one context planning all channels would find;
+ * the wideband plan's bins are gathered into kbin and its etab noted, the plan itself is rebuilt by the caller.
+ * to part: the part's channels are taken out, and its wideband plan is rebuilt from the full plan's bins. */
+static void chan_record(const MvHead &h, const MvLayout &F, const MvLayout &P, int c0, int nc, int nch, bool first, uint8_t *part,
+                        uint8_t *full, bool to_full, std::vector<int> &kbin, int &etab)
+{
+	auto mv = [to_full](uint8_t *p, uint8_t *f, size_t n) { to_full ? memcpy(f, p, n) : memcpy(p, f, n); };
+	MvRecHead ph, fh;
+	memcpy(&ph, part, sizeof(ph));
+	memcpy(&fh, full, sizeof(fh));
+	if (to_full) {
+		if (first) fh = MvRecHead{ ph.pos, ph.carry, fh.fast_ok, 0, 0 };
+		fh.fast_ok &= ph.fast_ok;
+		memcpy(full, &fh, sizeof(fh));
+	} else {
+		memcpy(part, &fh, sizeof(fh));
+	}
+	const int N2 = h.K / 4;
+	for (int k = 0; k < F.nreg; k++) {
+		uint8_t *fr = full + F.off[k], *pr = part + P.off[k];
+		switch (F.tag[k]) {
+		case acb::R_STATE: mv(pr, fr + (size_t)c0 * sizeof(acb::ChainState), (size_t)nc * sizeof(acb::ChainState)); break;
+		case acb::R_LCARRY: mv(pr, fr + (size_t)c0 * sizeof(acb::LevelCarry), (size_t)nc * sizeof(acb::LevelCarry)); break;
+		case acb::R_IN:
+			if (!to_full || first) mv(pr, fr, F.bytes[k]);
+			break;
+		case acb::R_WF: {                            /* [group][tap][8 channels] (c, d) */
+			const size_t fg = (size_t)(nch + 7) / 8, tp = F.bytes[k] / (fg * acb::CH_GROUP * 2 * sizeof(float));
+			for (int c = 0; c < nc; c++) {
+				const int g = c0 + c;
+				for (size_t t = 0; t < tp; t++)
+					mv(pr + (((size_t)(c / 8) * tp + t) * 8 + c % 8) * 8, fr + (((size_t)(g / 8) * tp + t) * 8 + g % 8) * 8, 8);
+			}
+			break;
+		}
+		case acb::R_TW:                              /* [group][8 channels][K/4] (Tr, Ti): channel-major */
+			mv(pr, fr + (size_t)c0 * N2 * 2 * sizeof(float), (size_t)nc * N2 * 2 * sizeof(float));
+			break;
+		case acb::R_TWMETA: {                        /* per group: 2-bit k mod 4 at 2*slot, 2-bit (k/2) mod 4 at 16 + 2*slot */
+			uint32_t *pw = (uint32_t *)pr, *fw = (uint32_t *)fr;
+			if (!to_full) memset(pr, 0, P.bytes[k]);
+			for (int c = 0; c < nc; c++) {
+				const int g = c0 + c;
+				const uint32_t *sw = to_full ? &pw[c / 8] : &fw[g / 8];
+				uint32_t *dw = to_full ? &fw[g / 8] : &pw[c / 8];
+				const int ss = to_full ? c % 8 : g % 8, ds = to_full ? g % 8 : c % 8;
+				for (int b : { 0, 16 }) {
+					const uint32_t v = (*sw >> (b + 2 * ss)) & 3u;
+					*dw = (*dw & ~(3u << (b + 2 * ds))) | (v << (b + 2 * ds));
+				}
+			}
+			break;
+		}
+		case acb::R_WBMETA: {
+			if (to_full) {
+				for (size_t z = 0; z < P.bytes[k] / (acb::WB_META * sizeof(int)); z++) {
+					const int *pm = (const int *)pr + z * acb::WB_META;
+					etab = pm[1];
+					for (int j = 0; j < std::min(pm[0] * acb::WB_CB, acb::WB_SLOTS); j++)     /* the slots in use only */
+						if (pm[3 + 2 * j] >= 0 && pm[3 + 2 * j] < nc) kbin[c0 + pm[3 + 2 * j]] = pm[2 + 2 * j];
+				}
+			} else {
+				acb::wb_meta(h.in_kind, nc, kbin.data() + c0, etab, (int *)pr);
+			}
+			break;
+		}
+		}
+	}
+	if (h.flags & ACB_FLAG_DECODE_STATS)
+		mv(part + P.off_dstats, full + F.off_dstats + (size_t)c0 * sizeof(acb_decode_stats_t), (size_t)nc * sizeof(acb_decode_stats_t));
+	if (h.flags & ACB_FLAG_LEVEL_STATS) {
+		if (!to_full || first) mv(part + P.off_lin, full + F.off_lin, sizeof(acb_input_level_t));
+		mv(part + P.off_lch, full + F.off_lch + (size_t)c0 * sizeof(acb_chan_level_t), (size_t)nc * sizeof(acb_chan_level_t));
+	}
+}
+
+/* the bins of a full record's wideband plan (0 for a stream not on the raster, whose plan is unused) */
+static void wb_bins(const MvLayout &F, const uint8_t *full, int nch, std::vector<int> &kbin, int &etab)
+{
+	MvRecHead fh;
+	memcpy(&fh, full, sizeof(fh));
+	std::fill(kbin.begin(), kbin.end(), 0);
+	for (int k = 0; k < F.nreg; k++) {
+		if (F.tag[k] != acb::R_WBMETA) continue;
+		for (size_t z = 0; z < F.bytes[k] / (acb::WB_META * sizeof(int)); z++) {
+			const int *fm = (const int *)(full + F.off[k]) + z * acb::WB_META;
+			etab = fm[1];
+			for (int j = 0; fh.fast_ok && j < std::min(fm[0] * acb::WB_CB, acb::WB_SLOTS); j++)     /* the slots in use only */
+				if (fm[3 + 2 * j] >= 0 && fm[3 + 2 * j] < nch) kbin[fm[3 + 2 * j]] = fm[2 + 2 * j];
+		}
+	}
+}
+
+/* the full layout: part 0's fingerprint (every part's but nch) with all of cfg's channels */
+static MvHead full_head(acb_multi *m)
+{
+	MvHead h;
+	acb::mv_fingerprint(m->parts[0].ctx, h);
+	h.nch = m->cfg.nch;
+	h.record_bytes = layout_of(h, h.nch).rec_bytes;
+	return h;
+}
+
+extern "C" size_t acb_multi_streams_blob_bytes(acb_multi_t *m, int n)
+{
+	if (!m || n < 1) return 0;
+	return acb::MV_HEAD_BYTES + (size_t)n * full_head(m).record_bytes;
+}
+
+/* Each part saves its streams (collecting its own submits in flight; their messages wait in the part's queue until the
+ * next acb_multi_collect / acb_multi_sync merges them), and the records go to their places in the caller's order */
+extern "C" int acb_multi_save_streams(acb_multi_t *m, const int *streams, int n, void *blob, size_t cap)
+{
+	if (!m || !blob) return fail(ACB_ERR_ARG, "null argument");
+	if (int r = multi_list(m, streams, n)) return r;
+	const MvHead h = full_head(m);
+	const MvLayout F = layout_of(h, h.nch);
+	const size_t rec = F.rec_bytes, need = acb::MV_HEAD_BYTES + (size_t)n * rec;
+	if (cap < need) return fail(ACB_ERR_ARG, "cap=%zu < %zu bytes", cap, need);
+	uint8_t *const out = (uint8_t *)blob, *const recs = out + acb::MV_HEAD_BYTES;
+	memcpy(out, &h, sizeof(h));
+	std::vector<uint8_t> tmp;
+	if (m->mode == ACB_MULTI_SPLIT_STREAMS) {
+		for (size_t p = 0; p < m->parts.size(); p++) {
+			std::vector<int> local, where;
+			for (int i = 0; i < n; i++)
+				if (part_of(m, streams[i]) == p) local.push_back(streams[i] - m->parts[p].s0), where.push_back(i);
+			if (local.empty()) continue;
+			tmp.resize(acb::MV_HEAD_BYTES + local.size() * rec);
+			if (int r = acb_save_streams(m->parts[p].ctx, local.data(), (int)local.size(), tmp.data(), tmp.size())) return r;
+			for (size_t j = 0; j < local.size(); j++)
+				memcpy(recs + (size_t)where[j] * rec, tmp.data() + acb::MV_HEAD_BYTES + j * rec, rec);
+		}
+	} else {
+		memset(recs, 0, (size_t)n * rec);
+		for (int i = 0; i < n; i++) {
+			MvRecHead fh{ 0, 0, 1, 0, 0 };
+			memcpy(recs + (size_t)i * rec, &fh, sizeof(fh));
+		}
+		std::vector<std::vector<int>> kbin(n, std::vector<int>(m->cfg.nch, 0));
+		std::vector<int> etab(n, 0);
+		for (size_t p = 0; p < m->parts.size(); p++) {
+			const Part &q = m->parts[p];
+			const MvLayout P = layout_of(h, q.nc);
+			tmp.resize(acb::MV_HEAD_BYTES + (size_t)n * P.rec_bytes);
+			if (int r = acb_save_streams(q.ctx, streams, n, tmp.data(), tmp.size())) return r;
+			for (int i = 0; i < n; i++)
+				chan_record(h, F, P, q.c0, q.nc, m->cfg.nch, p == 0, tmp.data() + acb::MV_HEAD_BYTES + (size_t)i * P.rec_bytes,
+				            recs + (size_t)i * rec, true, kbin[i], etab[i]);
+		}
+		for (int k = 0; k < F.nreg; k++) {
+			if (F.tag[k] != acb::R_WBMETA) continue;
+			for (int i = 0; i < n; i++) {
+				MvRecHead fh;
+				memcpy(&fh, recs + (size_t)i * rec, sizeof(fh));
+				if (!fh.fast_ok) std::fill(kbin[i].begin(), kbin[i].end(), 0);     /* not on the raster: the plan is unused */
+				acb::wb_meta(h.in_kind, m->cfg.nch, kbin[i].data(), etab[i], (int *)(recs + (size_t)i * rec + F.off[k]));
+			}
+		}
+	}
+	acb::mv_seal(out, need, n);
+	return ACB_OK;
+}
+
+/* Every part's records are made into a blob of its own and checked against that part before anything changes; then the
+ * submits in flight are collected (as acb_multi_reset_stream: the merge tells a message's submit by its stream's
+ * position), each part loads, and each stream's position becomes the record's */
+extern "C" int acb_multi_load_streams(acb_multi_t *m, const int *streams, int n, const void *blob, size_t size)
+{
+	if (!m || !blob) return fail(ACB_ERR_ARG, "null argument");
+	if (int r = multi_list(m, streams, n)) return r;
+	acb_streams_blob_info_t info;
+	if (int r = acb_streams_blob_check(blob, size, &info)) return r;
+	if (info.nch != m->cfg.nch || info.count != n) return fail(ACB_ERR_ARG, "blob of %d channels and %d records, the call %d and %d", info.nch,
+	                                                          info.count, m->cfg.nch, n);
+	MvHead h;
+	memcpy(&h, blob, sizeof(h));
+	const MvLayout F = layout_of(h, h.nch);
+	const uint8_t *const in = (const uint8_t *)blob + acb::MV_HEAD_BYTES;
+	std::vector<std::vector<uint8_t>> pb(m->parts.size());
+	std::vector<std::vector<int>> local(m->parts.size());
+	std::vector<int> kbin(m->cfg.nch);
+	for (size_t p = 0; p < m->parts.size(); p++) {
+		const Part &q = m->parts[p];
+		const MvLayout P = layout_of(h, q.nc);
+		MvHead ph = h;
+		ph.nch = q.nc;
+		ph.record_bytes = P.rec_bytes;
+		pb[p].assign((const uint8_t *)&ph, (const uint8_t *)&ph + sizeof(ph));
+		for (int i = 0; i < n; i++) {
+			if (m->mode == ACB_MULTI_SPLIT_STREAMS) {
+				if (part_of(m, streams[i]) != p) continue;
+				pb[p].insert(pb[p].end(), in + (size_t)i * F.rec_bytes, in + (size_t)(i + 1) * F.rec_bytes);
+			} else {
+				int etab = 0;
+				wb_bins(F, in + (size_t)i * F.rec_bytes, m->cfg.nch, kbin, etab);
+				const size_t at = pb[p].size();
+				pb[p].resize(at + P.rec_bytes, 0);
+				chan_record(h, F, P, q.c0, q.nc, m->cfg.nch, p == 0, pb[p].data() + at, const_cast<uint8_t *>(in + (size_t)i * F.rec_bytes),
+				            false, kbin, etab);
+			}
+			local[p].push_back(streams[i] - q.s0);
+		}
+		if (local[p].empty()) continue;
+		acb::mv_seal(pb[p].data(), pb[p].size(), (int)local[p].size());
+		if (int r = acb::mv_validate(q.ctx, pb[p].data(), pb[p].size(), (int)local[p].size())) return r;
+	}
+	const int r0 = acb_multi_sync(m);
+	if (r0 < 0) return r0;
+	for (size_t p = 0; p < m->parts.size(); p++)
+		if (!local[p].empty())
+			if (int r = acb_load_streams(m->parts[p].ctx, local[p].data(), (int)local[p].size(), pb[p].data(), pb[p].size())) return r;
+	for (int i = 0; i < n; i++) {
+		MvRecHead rh;
+		memcpy(&rh, in + (size_t)i * F.rec_bytes, sizeof(rh));
+		m->spos[streams[i]] = rh.pos;
+	}
+	return ACB_OK;
+}

@@ -455,9 +455,62 @@ int   acb_copy_to_device(acb_ctx_t *ctx, void *dst_dev, const void *src_host, si
 /* Envelope samples the channelizer produced for the last submit: out[(s*nsamp+n)*nch + c]. */
 int acb_read_dm(acb_ctx_t *ctx, float *out, size_t nfloats);
 /* The state is the demodulator's and the frame synchroniser's only: a round trip does not carry the channelizer's input
- * side — the streaming front-ends' carried remainder, or the window history of a taps > K context. */
+ * side — the streaming front-ends' carried remainder, or the window history of a taps > K context — nor the stream's
+ * position, tables or statistics.  To move a whole stream use acb_save_streams / acb_load_streams below. */
 int acb_get_state(acb_ctx_t *ctx, int stream, int chn, acb_chan_state_t *out);
 int acb_set_state(acb_ctx_t *ctx, int stream, int chn, const acb_chan_state_t *in);
+
+/* ---- moving streams: a stream's whole decoding state, to another slot, context, device or process ----
+ *
+ * A blob holds `count` records behind a 64-byte header; record i is one stream's state:
+ *   - its position (envelope rows since its start), carried remainder count and whether its plan is on the raster;
+ *   - its nch chain states (the frame being assembled, the PLL, the bit clock);
+ *   - the channelizer's input side: the u8 taps > K history, or the streaming kinds' history and carried remainder;
+ *   - its channel tables and fast plan, copied as the context holds them (no replanning);
+ *   - with ACB_FLAG_DECODE_STATS its decode counts, with ACB_FLAG_LEVEL_STATS its level tables and open 1024-row windows.
+ * Records have one size per configuration.  The exact tables dominate it: nch * taps_pad * 8 bytes (taps_pad: taps
+ * rounded up to 16 bytes of input), e.g. about 52 MB per stream at K = 1600, 256 channels, taps = 16K.
+ * The format is little-endian and opaque; it carries a magic, a format version, the fingerprint below and a CRC-32, and
+ * moves between builds of the same format version.
+ *
+ * The promise: stream s saved from one context and loaded into stream t of another, then fed what s would have been fed,
+ * gives bit for bit what s would have given had it stayed — envelope rows, messages (every field but `stream`), chain
+ * states, decode and level statistics, emission group numbers.  It holds for every input kind and channelizer form,
+ * taps = K and taps > K, lockstep and ragged, host and device submits, the same or another device or process.  One
+ * condition: both contexts must run the same channelizer form for the rows compared.  The fast forms run only while
+ * every stream of a context is planned on the raster (otherwise the whole context runs EXACT), so a stream's envelope
+ * can depend on its neighbours' plans; under a fast flag, give both contexts raster plans (or neither). */
+/* bytes a blob of n streams of this context takes */
+size_t acb_streams_blob_bytes(acb_ctx_t *ctx, int n);
+/* Save streams[0..n) into blob (cap >= acb_streams_blob_bytes(ctx, n)); record i is streams[i].  The submits in flight
+ * are collected first, as acb_sync collects them (their messages wait in the output queue, their counts are added; a
+ * ring overflow is left for the next acb_collect / acb_sync to report), so the blob holds each stream's state after every
+ * submit made so far, and a continuation produces only later messages.  The context is not changed.  To move a stream:
+ * save it, load it elsewhere, then stop feeding (or acb_reset_stream) the source slot.  Returns ACB_OK. */
+int acb_save_streams(acb_ctx_t *ctx, const int *streams, int n, void *blob, size_t cap);
+/* Load record i of blob into stream streams[i]: n must be the blob's record count, streams distinct and in range.  Like
+ * acb_reset_stream the load is queued behind the work in flight and touches no other stream: submits made before it
+ * still deliver that slot's messages (not their counts), and the slot's statistics become the blob's.  The bytes are
+ * staged before the call returns (the caller may free the blob); the host waits only for an earlier load's staging,
+ * and, when a save or load needs more staging than the context has used so far, for the allocation (which synchronises
+ * the device: save or load the largest set once up front to avoid it in a live pipeline).
+ * Refused with ACB_ERR_ARG, the context unchanged, unless the format version and the CRC match, and the input kind, K,
+ * taps, nch, channelizer form, the ACB_FLAG_DECODE_STATS and ACB_FLAG_LEVEL_STATS bits and (streaming kinds) the
+ * emission-group unit and period match the context's.  nstreams, max_blocks and the device may differ. */
+int acb_load_streams(acb_ctx_t *ctx, const int *streams, int n, const void *blob, size_t size);
+/* A blob's fingerprint; host only (no device, no context).  ACB_ERR_ARG for a wrong magic or version, a size that does
+ * not match the header, or a CRC mismatch. */
+typedef struct {
+	int in_kind;              /* 0 u8 IQ, 1 real, 2 CS16 */
+	int K, taps, nch;         /* taps as the context runs it (K for taps = 0) */
+	int form;                 /* the channelizer form: 0 EXACT, 1 GENERIC, 2 DFT, 3 RDFT, 4 OVL_FAST, 5 OVL_RDFT, 6 WB, 7 WB_REAL */
+	int flags;                /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS bits of the context */
+	int group_unit;           /* streaming kinds: ACB_GROUP_*; u8: 0 */
+	uint64_t group_period;
+	int count;                /* records */
+	uint64_t record_bytes;
+} acb_streams_blob_info_t;
+int acb_streams_blob_check(const void *blob, size_t size, acb_streams_blob_info_t *out);
 
 /* CUDA-event stopwatch on the context's compute stream (the stream the kernels run on):
  * acb_mark(ctx,0) ... submits ... acb_mark(ctx,1); acb_elapsed_ms waits for mark 1. */
@@ -613,6 +666,19 @@ int  acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *out, size_t 
 /* acb_get_level_stats over the parts, indexed globally.  A stream split takes each part's streams.  In a channel split
  * every part reads the same samples, so in[] comes from part 0; ch[] from each part's channels. */
 int  acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset);
+/* acb_save_streams / acb_load_streams over the parts.  A blob is the one a single context of cfg would give, whatever the
+ * split, so streams move freely between single contexts, stream splits and channel splits.  A stream split takes each
+ * stream's record from (gives it to) the part that owns it.  A channel split assembles each stream's nch chains, tables
+ * and counts from the parts' channels, and the input side and input levels from part 0 (every part reads the same
+ * samples); a stream is on the raster only when every part's channels are.  The envelope level sums of a channel split
+ * (acb_chan_level_t power_sum and floor, and the open windows' sums) follow its parts' channel tiling, as
+ * acb_multi_get_level_stats's do: within 1e-10 relative of a single context's, everything else bit for bit.  Load checks
+ * every part's share before any
+ * part changes, collects the submits in flight first (as acb_multi_reset_stream) and sets each stream's position to
+ * the blob's. */
+size_t acb_multi_streams_blob_bytes(acb_multi_t *m, int n);
+int  acb_multi_save_streams(acb_multi_t *m, const int *streams, int n, void *blob, size_t cap);
+int  acb_multi_load_streams(acb_multi_t *m, const int *streams, int n, const void *blob, size_t size);
 
 /* Block FEC on one frame in place on the HOST (acars.c:123-207): 1 = deliver, 0 = drop.  The
  * processing path runs the same repair on the device (k_block_fec, one thread per frame, right

@@ -155,4 +155,21 @@ for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
             ctx.submit_tensor(dev, counts=[n, 5, Kd + 1])
         ctx.sync()
         ctx.level_stats()
+# moving streams: k_stream_pack / k_stream_unpack over every region kind (chain states, the u8 history, the streaming
+# carry, exact tables, the fast plans' 4-byte-strided metadata, the open level windows), two streams to two other slots
+for kind, Kd, fl, tp in (("u8", K, 1 | 16 | api.FLAG_LEVEL_STATS, 2 * K + 3), ("cs16", K, 4 | 64, 0), ("real", Ka, 2 | 8, 0)):
+    with api.Context(Kd, 3, 3, 1, flags=fl, taps=tp) as a, api.Context(Kd, 4, 3, 1, flags=fl, taps=tp) as b:
+        for ctx in (a, b):
+            for s in range(ctx.nstreams):
+                (ctx.set_plan(s, fd[:3]) if kind == "u8" else ctx.set_plan_air(s, fda) if kind == "real"
+                 else ctx.set_plan_cs16(s, fd[:3], 0))
+        if kind == "u8":
+            dev = torch.randint(0, 256, (3, 1024 * Kd * 2), dtype=torch.uint8, device="cuda")
+            a.submit_device(dev.data_ptr(), 1, dev.stride(0))
+        else:
+            n = 3 * Kd + 7
+            dev = torch.randn((3, n), device="cuda") if kind == "real" else torch.randint(-3000, 3000, (3, n, 2), dtype=torch.int16, device="cuda")
+            a.submit_tensor(dev)
+        b.load_streams([3, 0], a.save_streams([2, 0]))
+        b.sync()
 print("sanitize run ok", n1, n3, n4, n5)
