@@ -2253,6 +2253,9 @@ extern "C" int acb_save_streams(acb_ctx_t *c, const int *streams, int n, void *b
 	if (int r = mv_stage(c, lb + (size_t)n * rec)) return r;
 	memcpy(c->h_mv, streams, (size_t)n * sizeof(int));
 	CU(cudaMemcpyAsync(c->d_mv, c->h_mv, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, c->s_comp));
+	/* the pack writes each region's bytes only: the padding up to the next 16-byte offset would otherwise carry whatever
+	 * the staging buffer held before, and equal states would not give equal blobs */
+	CU(cudaMemsetAsync(c->d_mv + lb, 0, (size_t)n * rec, c->s_comp));
 	int launched = 0;
 	if (int r = launch_stream_move(mv_regions(c, L), (const int *)c->d_mv, n, c->d_mv + lb, rec, false, c->s_comp, launched))
 		return fail(ACB_ERR_CUDA, "stream pack launch: %s", cudaGetErrorString((cudaError_t)r));

@@ -141,11 +141,14 @@ with api.Context(K, 3, 3, 2, flags=1 | api.FLAG_LEVEL_STATS, taps=2 * K + 3) as 
     ctx.submit_dm(np.ones((3, 1500, 3), np.float32))
     ctx.sync()
     ctx.level_stats()
-for kind, Kd, fl in (("real", Ka, 2), ("cs16", K, 4), ("planar", K, 4)):
+# K = 161 and 162: stream 0's 3 rows and stream 2's 1 row are 3 * K * 4 and K * 4 bytes, which end 12 and 4 bytes (K = 161)
+# or 8 bytes (K = 162) past a 16-byte load, so k_level_in's scalar tail reads them
+for kind, Kd, fl in (("real", 162, 2), ("cs16", 161, 4), ("planar", 162, 4)):
     with api.Context(Kd, 3, 3, 1, flags=fl | api.FLAG_LEVEL_STATS) as ctx:
         for s in range(3):
             ctx.set_plan_air(s, fda) if kind == "real" else ctx.set_plan_cs16(s, fd[:3], 0)
         n = 3 * Kd + 7
+        assert {3 * Kd * 4 % 16, Kd * 4 % 16} & {4, 8, 12}
         dev = (torch.randn((3, n), device="cuda") * 0.5 if kind == "real"
                else torch.randint(-32768, 32767, (3, n, 2), dtype=torch.int16, device="cuda"))
         if kind == "planar":
