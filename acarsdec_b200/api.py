@@ -21,6 +21,7 @@ FLAG_FAST_WIDEBAND = 64          # ACB_FLAG_FAST_WIDEBAND: the fast forms for an
 FLAG_FAST_WIDEBAND_REAL = 128    # ACB_FLAG_FAST_WIDEBAND_REAL: the same for real input (air.c)
 FLAG_DECODE_STATS = 256          # ACB_FLAG_DECODE_STATS: per-chain decode statistics (Context.decode_stats)
 FLAG_LEVEL_STATS = 512           # ACB_FLAG_LEVEL_STATS: input and envelope levels (Context.level_stats)
+FLAG_FREQ_STATS = 1024           # ACB_FLAG_FREQ_STATS: per-chain carrier offsets (Context.freq_stats, freq_error)
 
 
 class Config(C.Structure):
@@ -102,6 +103,9 @@ CHAN_LEVEL_DTYPE = np.dtype([("rows", "<u8"), ("power_sum", "<f8"), ("peak", "<f
 # full-scale amplitude of each input kind's converted components: the mean input power in dBFS is
 # 10*log10(power_sum / samples / fs**2)
 FULL_SCALE = {"u8": 127.5, "cs16": 32768.0, "real": 1.0}
+# acb_chan_freq_t: one chain's half-row rotation sums, its planned RF frequency and its NCO step
+CHAN_FREQ_DTYPE = np.dtype([("pairs", "<u8"), ("s_re", "<f8"), ("s_im", "<f8"), ("mag_sum", "<f8"), ("power_sum", "<f8"),
+                            ("freq_hz", "<f8"), ("step", "<f8")])
 
 
 class BlobInfo(C.Structure):
@@ -208,6 +212,9 @@ ABI = [
     ("acb_multi_get_decode_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
     ("acb_multi_get_level_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_get_freq_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_multi_get_freq_stats", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    ("acb_freq_error", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("acb_streams_blob_bytes", C.c_size_t, [C.c_void_p, C.c_int]),
     ("acb_save_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
     ("acb_load_streams", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]),
@@ -249,6 +256,20 @@ def _check(lib, rc: int) -> int:
     if rc < 0:
         raise AcbError(f"acars_b200 error {rc}: {lib.acb_last_error().decode()}")
     return rc
+
+
+def freq_error(table: np.ndarray, K: int) -> dict:
+    """A freq_stats table (CHAN_FREQ_DTYPE, shape (nstreams, nch)) of a context with this K, through acb_freq_error:
+    offset_hz and coherence of shape (nstreams, nch), and each stream's ppm of shape (nstreams,).  A positive offset is
+    a carrier above its planned frequency, for every input kind."""
+    lib = load()
+    t = np.ascontiguousarray(table, dtype=CHAN_FREQ_DTYPE)
+    t = t.reshape(1, -1) if t.ndim == 1 else t
+    ns, nch = t.shape
+    off, coh, ppm = np.zeros((ns, nch)), np.zeros((ns, nch)), np.zeros(ns)
+    for s in range(ns):
+        _check(lib, lib.acb_freq_error(t[s].ctypes.data, nch, K, off[s].ctypes.data, coh[s].ctypes.data, ppm[s:].ctypes.data))
+    return {"offset_hz": off, "coherence": coh, "ppm": ppm}
 
 
 # ---- front-end planning (host; same results as initRtl) ----
@@ -761,6 +782,13 @@ class Context:
         _check(self.lib, self.lib.acb_get_level_stats(self.h, inp.ctypes.data, inp.size, ch.ctypes.data, ch.size, int(reset)))
         return inp, ch
 
+    def freq_stats(self, reset: bool = False) -> np.ndarray:
+        """Per-chain carrier rotation sums (FLAG_FREQ_STATS): a CHAN_FREQ_DTYPE array of shape (nstreams, nch); freq_error
+        turns it into offsets and ppm."""
+        out = np.zeros((self.nstreams, self.nch), dtype=CHAN_FREQ_DTYPE)
+        _check(self.lib, self.lib.acb_get_freq_stats(self.h, out.ctypes.data, out.size, int(reset)))
+        return out
+
     def device_alloc(self, nbytes: int) -> int:
         p = self.lib.acb_device_alloc(self.h, nbytes)
         if not p:
@@ -921,6 +949,12 @@ class MultiContext:
         ch = np.zeros((self.nstreams, self.nch), dtype=CHAN_LEVEL_DTYPE)
         _check(self.lib, self.lib.acb_multi_get_level_stats(self.h, inp.ctypes.data, inp.size, ch.ctypes.data, ch.size, int(reset)))
         return inp, ch
+
+    def freq_stats(self, reset: bool = False) -> np.ndarray:
+        """As Context.freq_stats, indexed by global stream and channel."""
+        out = np.zeros((self.nstreams, self.nch), dtype=CHAN_FREQ_DTYPE)
+        _check(self.lib, self.lib.acb_multi_get_freq_stats(self.h, out.ctypes.data, out.size, int(reset)))
+        return out
 
     def part_input_levels(self, i: int) -> np.ndarray:
         """The input table of the i-th per-device context: its streams first (in a channel split, every stream)."""

@@ -173,6 +173,17 @@ int launch_level_input(int in_kind, const uint8_t *in, size_t stride, int K, int
                        LevelPart *part, size_t part_stride, LevelIn *out, CUstream_st *stream, int &launched);
 int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int nstreams, double *seg_sum, float *seg_peak,
                     int seg_stride, LevelCarry *carry, LevelChan *out, CUstream_st *stream, int &launched);
+/* ACB_FLAG_FREQ_STATS.  k_freq_in: one CTA per (FREQ_ROWS-row chunk, stream, 8-chain tile); each row's own K samples
+ * (the same `in`, `stride`, `rows` as launch_level_input) against nco[(s * nch + c) * K + n] ((re, im) float pairs,
+ * the chain's cos - j sin table), each chunk's sums per chain to part[(s * part_stride + chunk) * nch + c]; a final pass adds each
+ * chain's chunks in order into out[s * nch + c], zero for chains with on[g] == 0.  Returns a cudaError_t. */
+constexpr int FREQ_ROWS = 128;
+struct FreqPart { double re, im, mag, pow; };
+/* one submit's sums, laid out as the head of acb_chan_freq_t (context.cu checks it) */
+struct FreqChan { unsigned long long pairs; double s_re, s_im, mag_sum, power_sum; };
+int launch_freq_input(int in_kind, const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nch, int nstreams,
+                      const float *nco, const int *on, FreqPart *part, size_t part_stride, FreqChan *out, CUstream_st *stream,
+                      int &launched);
 /* Moving streams: each stream's device state is up to SP_MAXREG regions, stream s's `bytes` (a multiple of 4) at
  * base + s*stride, placed at `off` (a multiple of 16) in its record.  launch_stream_move copies list[i]'s regions to
  * (unpack = false: k_stream_pack) or from (true: k_stream_unpack) record i at rec + i*rec_bytes, in one launch; it fills
@@ -200,14 +211,14 @@ struct MvHead {
 static_assert(sizeof(MvHead) == 64, "the blob header is 64 bytes");
 struct MvRecHead { uint64_t pos, carry; uint32_t fast_ok, pad; uint64_t pad2; };
 static_assert(sizeof(MvRecHead) == 32, "the record's host part is 32 bytes");
-constexpr int MV_FLAGS = 256 | 512;            /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS */
+constexpr int MV_FLAGS = 256 | 512 | 1024;     /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS | ACB_FLAG_FREQ_STATS */
 enum MvRegion { R_STATE, R_IN, R_WF, R_TW, R_TWMETA, R_WBMETA, R_LCARRY };
 /* A record of a configuration: its device regions (tag, offset, bytes) in order, then the statistics' offsets */
 struct MvLayout {
 	int nreg;
 	int tag[SP_MAXREG];
 	size_t off[SP_MAXREG], bytes[SP_MAXREG];
-	size_t off_dstats, off_lin, off_lch, rec_bytes;
+	size_t off_dstats, off_lin, off_lch, off_fch, rec_bytes;
 };
 MvLayout mv_layout(int in_kind, int K, int taps, int nch, int form, int flags);
 /* a blob header of this context's configuration: magic, version and fingerprint (count and CRC left 0) */

@@ -184,7 +184,7 @@ struct acb_ctx {
 	 * level kernels on the channelizer stream (behind K1) and read back with that submit's frames; the consumer adds them to
 	 * lin / lch.  The open windows' carry (d_lcarry) is device state in submit order, on the channelizer stream. */
 	bool level_stats;
-	std::mutex lstats_mtx;       /* guards lin, lch, lstats_from */
+	std::mutex lstats_mtx;       /* guards lin, lch, lstats_from, fch */
 	LevelIn *d_lin[NPIPE], *h_lin[NPIPE];         /* [stream] (h_* pinned) */
 	LevelChan *d_lch[NPIPE], *h_lch[NPIPE];       /* [chain] */
 	cudaEvent_t ev_lvl_done[NPIPE];               /* behind the level kernels of the submit using ring b */
@@ -195,7 +195,18 @@ struct acb_ctx {
 	LevelCarry *d_lcarry;                         /* [chain] */
 	std::vector<acb_input_level_t> lin;           /* guarded by lstats_mtx */
 	std::vector<acb_chan_level_t> lch;
-	std::vector<unsigned long long> lstats_from;  /* per stream: the first submit its levels cover (acb_reset_stream) */
+	std::vector<unsigned long long> lstats_from;  /* per stream: the first submit its levels and frequency sums cover */
+	/* ACB_FLAG_FREQ_STATS: the same rings, event, read-back and consumer as the level statistics (dev_stats: either flag);
+	 * the sums are added to fch under lstats_mtx.  fch also holds each chain's plan (freq_hz, step), and d_fnco / d_fon
+	 * its NCO table and whether it is measured. */
+	bool freq_stats;
+	bool dev_stats;                               /* level_stats || freq_stats: the kernels behind K1 and their read-back */
+	float *d_fnco;                                /* [stream][nch][K] (re, im) */
+	int *d_fon;                                   /* [chain] */
+	FreqPart *d_fpart;                            /* [stream][fpart_stride][nch] */
+	size_t fpart_stride;
+	FreqChan *d_fch[NPIPE], *h_fch[NPIPE];        /* [chain] (h_* pinned) */
+	std::vector<acb_chan_freq_t> fch;             /* guarded by lstats_mtx */
 	int *d_rag[NRAG], *h_rag[NRAG];               /* ragged submits' counts (h_rag pinned) */
 	cudaEvent_t ev_rag_used[NRAG][3];             /* behind the last reads of slot i on the copy, channelizer and demod streams */
 	bool rag_used[NRAG];
@@ -265,6 +276,12 @@ static int sync_streams(acb_ctx *c)
 	return ACB_OK;
 }
 
+/* the sums of n chains; their plan (freq_hz, step) stays */
+static void clear_freq_sums(acb_chan_freq_t *t, size_t n)
+{
+	for (size_t i = 0; i < n; i++) t[i] = acb_chan_freq_t{ 0, 0.0, 0.0, 0.0, 0.0, t[i].freq_hz, t[i].step };
+}
+
 static int reset_states(acb_ctx *c)
 {
 	const size_t n = (size_t)c->cfg.nstreams * c->cfg.nch;
@@ -304,6 +321,10 @@ static int reset_states(acb_ctx *c)
 		std::lock_guard<std::mutex> lk(c->lstats_mtx);
 		memset(c->lin.data(), 0, c->lin.size() * sizeof(acb_input_level_t));
 		memset(c->lch.data(), 0, c->lch.size() * sizeof(acb_chan_level_t));
+	}
+	if (c->freq_stats) {
+		std::lock_guard<std::mutex> lk(c->lstats_mtx);
+		clear_freq_sums(c->fch.data(), c->fch.size());
 	}
 	c->overflowed = false;
 	return ACB_OK;
@@ -390,6 +411,12 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 	c->d_lseg_sum = nullptr;
 	c->d_lseg_peak = nullptr;
 	c->d_lcarry = nullptr;
+	c->freq_stats = (cfg->flags & ACB_FLAG_FREQ_STATS) != 0;
+	c->dev_stats = c->level_stats || c->freq_stats;
+	c->d_fnco = nullptr;
+	c->d_fon = nullptr;
+	c->d_fpart = nullptr;
+	for (int i = 0; i < NPIPE; i++) c->d_fch[i] = c->h_fch[i] = nullptr;
 	c->d_mv = c->h_mv = nullptr;
 	c->mv_cap = 0;
 	c->ev_mv = nullptr;
@@ -532,13 +559,11 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		const int ns = cfg->nstreams;
 		c->lin.assign(ns, acb_input_level_t{});
 		c->lch.assign(nchain, acb_chan_level_t{});
-		c->lstats_from.assign(ns, 0);
 		for (int i = 0; i < NPIPE; i++) {
 			CU(cudaMalloc(&c->d_lin[i], ns * sizeof(LevelIn)));
 			CU(cudaHostAlloc(&c->h_lin[i], ns * sizeof(LevelIn), cudaHostAllocDefault));
 			CU(cudaMalloc(&c->d_lch[i], nchain * sizeof(LevelChan)));
 			CU(cudaHostAlloc(&c->h_lch[i], nchain * sizeof(LevelChan), cudaHostAllocDefault));
-			CU(cudaEventCreateWithFlags(&c->ev_lvl_done[i], cudaEventDisableTiming));
 		}
 		/* a stream's rows of one submit: at most max_blocks * 1024 rows of K samples */
 		const size_t in_bytes_max = (size_t)cfg->max_blocks * OUTBLK * cfg->K * (c->in_kind == IN_KIND_U8IQ ? 2 : 4);
@@ -548,6 +573,26 @@ extern "C" int acb_create(const acb_config_t *cfg, acb_ctx_t **out)
 		CU(cudaMalloc(&c->d_lseg_sum, nseg * sizeof(double)));
 		CU(cudaMalloc(&c->d_lseg_peak, nseg * sizeof(float)));
 		CU(cudaMalloc(&c->d_lcarry, nchain * sizeof(LevelCarry)));
+	}
+	if (c->freq_stats) {
+		static_assert(sizeof(FreqChan) == offsetof(acb_chan_freq_t, freq_hz) && offsetof(FreqChan, power_sum) == offsetof(acb_chan_freq_t, power_sum),
+		              "FreqChan is the head of acb_chan_freq_t");
+		c->fch.assign(nchain, acb_chan_freq_t{});
+		for (int i = 0; i < NPIPE; i++) {
+			CU(cudaMalloc(&c->d_fch[i], nchain * sizeof(FreqChan)));
+			CU(cudaHostAlloc(&c->h_fch[i], nchain * sizeof(FreqChan), cudaHostAllocDefault));
+		}
+		c->fpart_stride = ((size_t)cfg->max_blocks * OUTBLK + FREQ_ROWS - 1) / FREQ_ROWS;
+		CU(cudaMalloc(&c->d_fpart, (size_t)cfg->nstreams * c->fpart_stride * cfg->nch * sizeof(FreqPart)));
+		CU(cudaMalloc(&c->d_fnco, nchain * cfg->K * 2 * sizeof(float)));
+		CU(cudaMalloc(&c->d_fon, nchain * sizeof(int)));
+		CU(cudaMemsetAsync(c->d_fnco, 0, nchain * cfg->K * 2 * sizeof(float), c->s_copy));
+		CU(cudaMemsetAsync(c->d_fon, 0, nchain * sizeof(int), c->s_copy));
+		CU(cudaStreamSynchronize(c->s_copy));
+	}
+	if (c->dev_stats) {
+		c->lstats_from.assign(cfg->nstreams, 0);
+		for (int i = 0; i < NPIPE; i++) CU(cudaEventCreateWithFlags(&c->ev_lvl_done[i], cudaEventDisableTiming));
 	}
 	c->rag_seq = 0;
 	for (int i = 0; i < NRAG; i++) {
@@ -609,6 +654,8 @@ extern "C" void acb_destroy(acb_ctx_t *c)
 			if (c->ev_lvl_done[i]) cudaEventDestroy(c->ev_lvl_done[i]);
 		}
 		cudaFree(c->d_lpart); cudaFree(c->d_lseg_sum); cudaFree(c->d_lseg_peak); cudaFree(c->d_lcarry);
+		for (int i = 0; i < NPIPE; i++) { cudaFree(c->d_fch[i]); cudaFreeHost(c->h_fch[i]); }
+		cudaFree(c->d_fpart); cudaFree(c->d_fnco); cudaFree(c->d_fon);
 		cudaFree(c->d_mv); cudaFreeHost(c->h_mv);
 		if (c->ev_mv) cudaEventDestroy(c->ev_mv);
 		for (int i = 0; i < NRAG; i++) {
@@ -665,10 +712,40 @@ extern "C" int acb_reset_stream(acb_ctx_t *c, int stream)
 	if (c->level_stats) {
 		/* the stream's open windows, behind the level kernels already queued on the channelizer stream */
 		CU(cudaMemsetAsync(c->d_lcarry + (size_t)stream * c->cfg.nch, 0, (size_t)c->cfg.nch * sizeof(LevelCarry), c->s_comp));
+	}
+	if (c->dev_stats) {
 		std::lock_guard<std::mutex> lk(c->lstats_mtx);
-		c->lin[stream] = acb_input_level_t{};
-		memset(&c->lch[(size_t)stream * c->cfg.nch], 0, (size_t)c->cfg.nch * sizeof(acb_chan_level_t));
+		if (c->level_stats) {
+			c->lin[stream] = acb_input_level_t{};
+			memset(&c->lch[(size_t)stream * c->cfg.nch], 0, (size_t)c->cfg.nch * sizeof(acb_chan_level_t));
+		}
+		if (c->freq_stats) clear_freq_sums(&c->fch[(size_t)stream * c->cfg.nch], c->cfg.nch);
 		c->lstats_from[stream] = c->nsubmit;
+	}
+	return ACB_OK;
+}
+
+/* ACB_FLAG_FREQ_STATS: stream s's chains are measured against freq[c] (0: not measured) with NCO step step[c]; the table
+ * is built in double and rounded to float once per entry.  Complete on return, like every table upload. */
+static int set_freq_plan(acb_ctx *c, int stream, const double *freq, const double *step)
+{
+	const int nch = c->cfg.nch, K = c->cfg.K;
+	std::vector<float> w((size_t)nch * K * 2);
+	std::vector<int> on(nch);
+	for (int ch = 0; ch < nch; ch++) {
+		on[ch] = freq[ch] > 0;
+		for (int n = 0; n < K; n++) {
+			const double ph = step[ch] * n;
+			w[((size_t)ch * K + n) * 2] = (float)cos(ph);
+			w[((size_t)ch * K + n) * 2 + 1] = -(float)sin(ph);
+		}
+	}
+	if (int r = upload(c, c->d_fnco + (size_t)stream * w.size(), w.data(), w.size() * sizeof(float))) return r;
+	if (int r = upload(c, c->d_fon + (size_t)stream * nch, on.data(), on.size() * sizeof(int))) return r;
+	std::lock_guard<std::mutex> lk(c->lstats_mtx);
+	for (int ch = 0; ch < nch; ch++) {
+		c->fch[(size_t)stream * nch + ch].freq_hz = freq[ch];
+		c->fch[(size_t)stream * nch + ch].step = step[ch];
 	}
 	return ACB_OK;
 }
@@ -692,6 +769,10 @@ extern "C" int acb_set_wf(acb_ctx_t *c, int stream, const float *wf, int nch)
 	if (int r = sync_streams(c)) return r;
 	if (int r = upload(c, c->d_wf + (size_t)stream * t.size(), t.data(), t.size() * sizeof(float))) return r;
 	c->fast_ok[stream] = 0;                     /* a caller's table has no known structure: exact kernel */
+	if (c->freq_stats) {                        /* nor a known frequency: not measured (the planners set it after this) */
+		const std::vector<double> zero(nch, 0.0);
+		return set_freq_plan(c, stream, zero.data(), zero.data());
+	}
 	return ACB_OK;
 }
 
@@ -755,13 +836,22 @@ static int upload_wb_plan(acb_ctx *c, int stream, const std::vector<int> &kbin, 
 /* The planners' common tail: the exact tables, `build(ch, wf)` writing channel ch's taps (the low-pass form at taps > K),
  * then the plan the context's form reads.  `plan(kbin, tw1)` is the input kind's acb_fast_plan* (tw1 NULL: the bins
  * only), 1 when every channel sits on the raster: otherwise the stream stays on EXACT.  `etab`: upload_wb_plan's. */
-template <class Build, class Plan>
-static int plan_stream(acb_ctx *c, int stream, const Build &build, const Plan &plan, int etab)
+template <class Build, class Plan, class Off>
+static int plan_stream(acb_ctx *c, int stream, const Build &build, const Plan &plan, int etab, double f0, const Off &off)
 {
 	const int nch = c->cfg.nch, T = c->taps;
 	std::vector<float> wf((size_t)nch * T * 2);
 	for (int ch = 0; ch < nch; ch++) build(ch, &wf[(size_t)ch * T * 2]);
 	if (int r = acb_set_wf(c, stream, wf.data(), nch)) return r;
+	if (c->freq_stats) {
+		/* the measurement mixes with the offset `off(ch)` Hz from f0 (see acb_chan_freq_t) */
+		std::vector<double> freq(nch), step(nch);
+		for (int ch = 0; ch < nch; ch++) {
+			freq[ch] = f0 + off(ch);
+			step[ch] = 2.0 * M_PI * off(ch) / ((double)ACB_INTRATE * c->cfg.K);
+		}
+		if (int r = set_freq_plan(c, stream, freq.data(), step.data())) return r;
+	}
 	if (c->form == CHAN_EXACT || c->form == CHAN_GENERIC) return ACB_OK;
 	std::vector<int> kbin(nch);
 	if (c->form == CHAN_WB || c->form == CHAN_WB_REAL) return plan(kbin.data(), nullptr) == 1 ? upload_wb_plan(c, stream, kbin, etab) : ACB_OK;
@@ -789,7 +879,8 @@ extern "C" int acb_set_plan_at(acb_ctx_t *c, int stream, const unsigned *freqs_h
 	return plan_stream(c, stream, [&](int ch, float *wf) {
 		if (c->hpad) acb_build_wf_lp(acb_stored_fr(freqs_hz[ch]), fc, K, T, wf);
 		else acb_build_wf(acb_stored_fr(freqs_hz[ch]), fc, K, wf);
-	}, [&](int *kbin, float *tw1) { return acb_fast_plan(freqs_hz, nch, K, fc, kbin, tw1); }, 0);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan(freqs_hz, nch, K, fc, kbin, tw1); }, 0,
+	(double)fc, [&](int ch) { return (double)((float)acb_stored_fr(freqs_hz[ch]) - (float)fc); });
 }
 
 static EvTriple get_events(acb_ctx *c)
@@ -875,6 +966,26 @@ static void add_level_stats(acb_ctx *c, const acb_ctx::Job &job)
 			d.peak = std::max(d.peak, e.peak);
 			if (e.windows) d.floor = d.windows ? std::min(d.floor, e.floor) : e.floor;
 			d.windows += e.windows;
+		}
+	}
+}
+
+/* ACB_FLAG_FREQ_STATS: a collected submit's sums into the context's table (envelope input measures nothing) */
+static void add_freq_stats(acb_ctx *c, const acb_ctx::Job &job)
+{
+	std::lock_guard<std::mutex> lk(c->lstats_mtx);
+	const int nch = c->cfg.nch;
+	const FreqChan *e = c->h_fch[job.ring];
+	for (int s = 0; s < c->cfg.nstreams; s++) {
+		if (job.seq < c->lstats_from[s]) continue;        /* made before the stream's acb_reset_stream */
+		for (int k = 0; k < nch; k++) {
+			const FreqChan &x = e[(size_t)s * nch + k];
+			acb_chan_freq_t &d = c->fch[(size_t)s * nch + k];
+			d.pairs += x.pairs;
+			d.s_re += x.s_re;
+			d.s_im += x.s_im;
+			d.mag_sum += x.mag_sum;
+			d.power_sum += x.power_sum;
 		}
 	}
 }
@@ -1014,6 +1125,7 @@ static void consume(acb_ctx *c, const acb_ctx::Job &job)
 	}
 	if (c->decode_stats) add_decode_stats(c, job, ring, keep.data());     /* before the job counts as done */
 	if (c->level_stats) add_level_stats(c, job);
+	if (c->freq_stats && job.chan) add_freq_stats(c, job);
 	const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
 	std::lock_guard<std::mutex> lk(c->mtx);
 	c->stats.raw_frames += count;
@@ -1037,7 +1149,7 @@ static void consumer_main(acb_ctx *c)
 			job = std::move(c->jobs.front());
 			c->jobs.pop_front();
 		}
-		const cudaError_t e = job.count || c->decode_stats || c->level_stats ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
+		const cudaError_t e = job.count || c->decode_stats || c->dev_stats ? cudaEventSynchronize(c->ev_ring_read[job.ring]) : cudaSuccess;
 		if (e == cudaSuccess) consume(c, job);
 		{
 			std::lock_guard<std::mutex> lk(c->mtx);
@@ -1084,11 +1196,14 @@ static int harvest_begin(acb_ctx *c)
 	if (c->decode_stats)           /* the submit's demod is done (ev.c follows it): its counters travel with its frames */
 		CU(cudaMemcpyAsync(c->h_evcnt[t.ring], c->d_evcnt[t.ring], c->dstats.size() * EV_COUNT * sizeof(unsigned),
 		                   cudaMemcpyDeviceToHost, c->s_d2h));
-	if (c->level_stats) {          /* the level kernels run on the channelizer stream: the copies wait for them */
+	if (c->dev_stats)              /* the level and frequency kernels run on the channelizer stream: the copies wait for them */
 		CU(cudaStreamWaitEvent(c->s_d2h, c->ev_lvl_done[t.ring], 0));
+	if (c->level_stats) {
 		CU(cudaMemcpyAsync(c->h_lin[t.ring], c->d_lin[t.ring], c->lin.size() * sizeof(LevelIn), cudaMemcpyDeviceToHost, c->s_d2h));
 		CU(cudaMemcpyAsync(c->h_lch[t.ring], c->d_lch[t.ring], c->lch.size() * sizeof(LevelChan), cudaMemcpyDeviceToHost, c->s_d2h));
 	}
+	if (c->freq_stats && t.ev.chan)
+		CU(cudaMemcpyAsync(c->h_fch[t.ring], c->d_fch[t.ring], c->fch.size() * sizeof(FreqChan), cudaMemcpyDeviceToHost, c->s_d2h));
 	CU(cudaEventRecord(c->ev_ring_read[t.ring], c->s_d2h));
 	c->ring_read_pending[t.ring] = true;
 	{
@@ -1109,21 +1224,26 @@ static int collect_oldest(acb_ctx *c)
 	return ACB_OK;
 }
 
-/* ACB_FLAG_LEVEL_STATS: the levels of the submit using ring b, on the channelizer stream: the input's (`in`, NULL for
- * envelope input) and the envelope's.  They write that ring's result buffers, so they wait until the read-back of the
- * submit that used it before is done. */
+/* ACB_FLAG_LEVEL_STATS / ACB_FLAG_FREQ_STATS: the statistics of the submit using ring b, on the channelizer stream: the
+ * input's levels and frequency sums (`in`, NULL for envelope input) and the envelope's levels.  They write that ring's
+ * result buffers, so they wait until the read-back of the submit that used it before is done. */
 static int run_level(acb_ctx *c, int b, const uint8_t *in, size_t stride, int nsamp, const int *rag)
 {
 	if (c->ring_read_pending[b]) CU(cudaStreamWaitEvent(c->s_comp, c->ev_ring_read[b], 0));
-	int launched = 0;
-	int r = in ? launch_level_input(c->in_kind, in, stride, c->cfg.K, nsamp, rag, c->cfg.nstreams, c->d_lpart, c->lpart_stride, c->d_lin[b],
-	                                c->s_comp, launched)
-	           : 0;
-	if (!r)
-		r = launch_level_dm(c->d_dm[b], nsamp, rag, c->cfg.nch, c->cfg.nstreams, c->d_lseg_sum, c->d_lseg_peak, c->cfg.max_blocks + 2,
-		                    c->d_lcarry, c->d_lch[b], c->s_comp, launched);
+	int launched = 0, r = 0;
+	if (c->level_stats) {
+		r = in ? launch_level_input(c->in_kind, in, stride, c->cfg.K, nsamp, rag, c->cfg.nstreams, c->d_lpart, c->lpart_stride, c->d_lin[b],
+		                            c->s_comp, launched)
+		       : 0;
+		if (!r)
+			r = launch_level_dm(c->d_dm[b], nsamp, rag, c->cfg.nch, c->cfg.nstreams, c->d_lseg_sum, c->d_lseg_peak, c->cfg.max_blocks + 2,
+			                    c->d_lcarry, c->d_lch[b], c->s_comp, launched);
+	}
+	if (!r && c->freq_stats && in)
+		r = launch_freq_input(c->in_kind, in, stride, c->cfg.K, nsamp, rag, c->cfg.nch, c->cfg.nstreams, c->d_fnco, c->d_fon, c->d_fpart,
+		                      c->fpart_stride, c->d_fch[b], c->s_comp, launched);
 	c->stats.kernel_launches += launched;
-	if (r) return fail(ACB_ERR_CUDA, "level launch: %s", cudaGetErrorString((cudaError_t)r));
+	if (r) return fail(ACB_ERR_CUDA, "statistics launch: %s", cudaGetErrorString((cudaError_t)r));
 	CU(cudaEventRecord(c->ev_lvl_done[b], c->s_comp));
 	return ACB_OK;
 }
@@ -1219,7 +1339,7 @@ static int run_kernels(acb_ctx *c, const uint8_t *d_iq, size_t stride, int nblk,
 		CU(cudaEventRecord(c->ev_k1_done[b], c->s_comp));
 		c->k1_pending[b] = true;
 		CU(cudaStreamWaitEvent(c->s_dem, c->ev_k1_done[b], 0));
-		if (c->level_stats) {
+		if (c->dev_stats) {
 			/* behind K1, beside the demod; the input-lifetime event moves behind them, as they read the input too */
 			if (int r2 = run_level(c, b, d_iq, stride, nsamp, rag)) return r2;
 			CU(cudaEventRecord(c->ev_k1_done[b], c->s_comp));
@@ -1741,7 +1861,8 @@ extern "C" int acb_set_plan_cs16(acb_ctx_t *c, int stream, const unsigned *freqs
 	return plan_stream(c, stream, [&](int ch, float *wf) {
 		if (c->hpad) acb_cs16_build_wf_lp(variant, freqs_hz[ch], fc, K, T, wf);
 		else acb_cs16_build_wf(variant, freqs_hz[ch], fc, K, wf);
-	}, [&](int *kbin, float *tw1) { return acb_fast_plan_cs16(variant, freqs_hz, nch, K, fc, kbin, tw1); }, variant);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan_cs16(variant, freqs_hz, nch, K, fc, kbin, tw1); }, variant,
+	(double)fc, [&](int ch) { return (double)((float)freqs_hz[ch] - (float)fc); });
 }
 
 static int check_plan_air(acb_ctx *c, const unsigned *freqs_hz, int nch)
@@ -1760,7 +1881,10 @@ static int plan_air(acb_ctx *c, int stream, const unsigned *freqs_hz, int nch, u
 	return plan_stream(c, stream, [&](int ch, float *wf) {
 		if (c->hpad) acb_air_build_wf_lp((int)freqs_hz[ch], (int)fc, rate, T, wf);
 		else acb_air_build_wf((int)freqs_hz[ch], (int)fc, rate, wf);
-	}, [&](int *kbin, float *tw1) { return acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin, tw1); }, 0);
+	}, [&](int *kbin, float *tw1) { return acb_fast_plan_air(freqs_hz, nch, c->cfg.K, fc, kbin, tw1); }, 0,
+	/* air.c's IF, Fc - Fr + rate/4, is the carrier's mirror image: the measurement mixes with its negative, where the
+	 * carrier turns the way its RF offset does */
+	(double)fc + rate / 4, [&](int ch) { return -(double)(unsigned)((int)fc - (int)freqs_hz[ch] + (int)(rate / 4)); });
 }
 
 extern "C" int acb_set_plan_air(acb_ctx_t *c, int stream, const unsigned *freqs_hz, int nch, unsigned *fc_out)
@@ -2031,12 +2155,42 @@ extern "C" int acb_get_level_stats(acb_ctx_t *c, acb_input_level_t *in, size_t n
 	return ACB_OK;
 }
 
+extern "C" int acb_get_freq_stats(acb_ctx_t *c, acb_chan_freq_t *out, size_t n, int reset)
+{
+	if (!c || !out) return fail(ACB_ERR_ARG, "null argument");
+	if (!c->freq_stats) return fail(ACB_ERR_ARG, "context was not created with ACB_FLAG_FREQ_STATS");
+	if (n < c->fch.size()) return fail(ACB_ERR_ARG, "n=%zu < nstreams*nch=%zu", n, c->fch.size());
+	std::lock_guard<std::mutex> lk(c->lstats_mtx);
+	memcpy(out, c->fch.data(), c->fch.size() * sizeof(acb_chan_freq_t));
+	if (reset) clear_freq_sums(c->fch.data(), c->fch.size());
+	return ACB_OK;
+}
+
+extern "C" int acb_freq_error(const acb_chan_freq_t *ch, int nch, int K, double *offset_hz, double *coherence, double *ppm)
+{
+	if (!ch || nch < 1 || K < 2) return fail(ACB_ERR_ARG, "null table, nch < 1 or K < 2");
+	const double scale = (double)ACB_INTRATE * K / (2.0 * M_PI * (K / 2));
+	double wsum = 0.0, wppm = 0.0;
+	for (int c = 0; c < nch; c++) {
+		const double mag = hypot(ch[c].s_re, ch[c].s_im);
+		const double off = ch[c].pairs ? scale * atan2(ch[c].s_im, ch[c].s_re) : 0.0;
+		if (offset_hz) offset_hz[c] = off;
+		if (coherence) coherence[c] = ch[c].pairs && ch[c].mag_sum > 0 ? mag / ch[c].mag_sum : 0.0;
+		if (ch[c].pairs && ch[c].freq_hz > 0) {
+			wsum += mag;
+			wppm += mag * off / ch[c].freq_hz;
+		}
+	}
+	if (ppm) *ppm = wsum > 0 ? 1e6 * wppm / wsum : 0.0;
+	return ACB_OK;
+}
+
 /* ---- moving streams (acb_save_streams / acb_load_streams) ----
  *
  * Blob: a 64-byte header (MvHead), then `count` records of record_bytes each.  A record is a 32-byte host part (MvRecHead),
  * the device regions of mv_layout at 16-byte aligned offsets (copied verbatim by k_stream_pack / k_stream_unpack), then
  * the host statistics: nch acb_decode_stats_t (ACB_FLAG_DECODE_STATS), one acb_input_level_t and nch acb_chan_level_t
- * (ACB_FLAG_LEVEL_STATS).  The CRC-32 (IEEE, as zlib's crc32) covers every byte from offset 16 to the end. */
+ * (ACB_FLAG_LEVEL_STATS), nch acb_chan_freq_t (ACB_FLAG_FREQ_STATS: the NCO tables are rebuilt from their steps).  The CRC-32 (IEEE, as zlib's crc32) covers every byte from offset 16 to the end. */
 namespace {
 constexpr char MV_MAGIC[8] = { 'A', 'C', 'B', 'S', 'T', 'R', 'M', 0 };
 /* The records copy these layouts verbatim, so a blob of one version means them: change any of them (a field moved, a
@@ -2048,8 +2202,8 @@ static_assert(sizeof(ChainState) == 432 && offsetof(ChainState, state) == 44 && 
               "ChainState changed: bump MV_VERSION");
 static_assert(sizeof(LevelCarry) == 16 && offsetof(LevelCarry, rows) == 8, "LevelCarry changed: bump MV_VERSION");
 static_assert(CH_GROUP == 8 && WB_CTILE == 256 && WB_CB == 4 && WB_META == 546, "table layouts changed: bump MV_VERSION");
-static_assert(sizeof(acb_decode_stats_t) == 120 && sizeof(acb_input_level_t) == 32 && sizeof(acb_chan_level_t) == 40,
-              "statistics changed: bump MV_VERSION");
+static_assert(sizeof(acb_decode_stats_t) == 120 && sizeof(acb_input_level_t) == 32 && sizeof(acb_chan_level_t) == 40 &&
+              sizeof(acb_chan_freq_t) == 56, "statistics changed: bump MV_VERSION");
 }
 
 static size_t round16(size_t x) { return (x + 15) & ~(size_t)15; }
@@ -2084,6 +2238,8 @@ MvLayout acb::mv_layout(int in_kind, int K, int taps, int nch, int form, int fla
 	L.off_lin = off;
 	L.off_lch = off + sizeof(acb_input_level_t);
 	if (flags & ACB_FLAG_LEVEL_STATS) off += sizeof(acb_input_level_t) + (size_t)nch * sizeof(acb_chan_level_t);
+	L.off_fch = off;
+	if (flags & ACB_FLAG_FREQ_STATS) off += (size_t)nch * sizeof(acb_chan_freq_t);
 	L.rec_bytes = round16(off);
 	return L;
 }
@@ -2287,6 +2443,10 @@ extern "C" int acb_save_streams(acb_ctx_t *c, const int *streams, int n, void *b
 			memcpy(r + L.off_lin, &c->lin[s], sizeof(acb_input_level_t));
 			memcpy(r + L.off_lch, &c->lch[(size_t)s * nch], (size_t)nch * sizeof(acb_chan_level_t));
 		}
+		if (c->freq_stats) {
+			std::lock_guard<std::mutex> lk(c->lstats_mtx);
+			memcpy(r + L.off_fch, &c->fch[(size_t)s * nch], (size_t)nch * sizeof(acb_chan_freq_t));
+		}
 	}
 	mv_seal(out, need, n);
 	return ACB_OK;
@@ -2381,10 +2541,23 @@ extern "C" int acb_load_streams(acb_ctx_t *c, const int *streams, int n, const v
 			memcpy(&c->dstats[(size_t)s * nch], r + L.off_dstats, (size_t)nch * sizeof(acb_decode_stats_t));
 			c->dstats_from[s] = c->nsubmit;
 		}
-		if (c->level_stats) {
+		if (c->freq_stats) {
+			/* the submits before the load are not counted for this stream (below), so the table may change under them */
+			std::vector<double> freq(nch), step(nch);
+			for (int ch = 0; ch < nch; ch++) {
+				acb_chan_freq_t f;
+				memcpy(&f, r + L.off_fch + (size_t)ch * sizeof(f), sizeof(f));
+				freq[ch] = f.freq_hz, step[ch] = f.step;
+			}
+			if (int e = set_freq_plan(c, s, freq.data(), step.data())) return e;
+		}
+		if (c->dev_stats) {
 			std::lock_guard<std::mutex> lk(c->lstats_mtx);
-			memcpy(&c->lin[s], r + L.off_lin, sizeof(acb_input_level_t));
-			memcpy(&c->lch[(size_t)s * nch], r + L.off_lch, (size_t)nch * sizeof(acb_chan_level_t));
+			if (c->level_stats) {
+				memcpy(&c->lin[s], r + L.off_lin, sizeof(acb_input_level_t));
+				memcpy(&c->lch[(size_t)s * nch], r + L.off_lch, (size_t)nch * sizeof(acb_chan_level_t));
+			}
+			if (c->freq_stats) memcpy(&c->fch[(size_t)s * nch], r + L.off_fch, (size_t)nch * sizeof(acb_chan_freq_t));
 			c->lstats_from[s] = c->nsubmit;
 		}
 	}

@@ -3875,6 +3875,159 @@ int launch_level_dm(const float *dm, int nrows, const int *rows, int nch, int ns
 	return (int)cudaGetLastError();
 }
 
+/* ---- ACB_FLAG_FREQ_STATS: each chain's carrier rotation between the two halves of a row (launch_freq_input) ----
+ * A row's half sums a = sum_{n<h} x[n] w[n] and b = sum_{n<h} x[h+n] w[h+n] (h = K/2, w the chain's NCO table) are a
+ * complex matrix product of the staged rows and the tables, in float with FMA; the row's terms b conj(a), |a||b| and
+ * |a|^2 + |b|^2 are formed in double.  Each warp owns one chain of a FQ_CT-chain tile and every row of a FQ_ROWS-row
+ * chunk (lane l: rows l, l + 32, l + 64, l + 96): the lane adds its rows in order, a butterfly adds the lanes, and the
+ * final pass adds the chunks in order.  That order depends on the row index alone, not on nch or on where a chain sits
+ * in its context, so a channel split gives a single context's bits. */
+constexpr int FQ_CT = 8;                         /* chains per CTA: one per warp */
+constexpr int FQ_RPL = FREQ_ROWS / 32;           /* rows per lane */
+constexpr int FQ_KT = 16;                        /* half-row samples staged per step */
+
+template <int KIND> struct FreqX { using T = float2; };
+template <> struct FreqX<IN_F32REAL> { using T = float; };
+
+/* sample n of a row, converted as the channelizer converts it */
+template <int KIND> __device__ __forceinline__ typename FreqX<KIND>::T freq_load(const uint8_t *row, int n)
+{
+	if constexpr (KIND == IN_U8IQ) {
+		const unsigned short v = *reinterpret_cast<const unsigned short *>(row + 2 * (size_t)n);
+		return make_float2((float)(v & 0xffu) - 127.37f, (float)(v >> 8) - 127.37f);
+	} else if constexpr (KIND == IN_CS16IQ) {
+		const unsigned v = *reinterpret_cast<const unsigned *>(row + 4 * (size_t)n);
+		return make_float2((float)(short)(v & 0xffffu), (float)((int)v >> 16));
+	} else {
+		return *reinterpret_cast<const float *>(row + 4 * (size_t)n);
+	}
+}
+
+__device__ __forceinline__ void freq_mac(float2 &acc, float2 x, float2 w)
+{
+	acc.x = fmaf(x.x, w.x, acc.x);
+	acc.x = fmaf(-x.y, w.y, acc.x);
+	acc.y = fmaf(x.x, w.y, acc.y);
+	acc.y = fmaf(x.y, w.x, acc.y);
+}
+__device__ __forceinline__ void freq_mac(float2 &acc, float x, float2 w)
+{
+	acc.x = fmaf(x, w.x, acc.x);
+	acc.y = fmaf(x, w.y, acc.y);
+}
+
+__device__ __forceinline__ void freq_shfl_add(FreqPart &v, int m)
+{
+	v.re = __dadd_rn(v.re, __shfl_xor_sync(0xffffffffu, v.re, m));
+	v.im = __dadd_rn(v.im, __shfl_xor_sync(0xffffffffu, v.im, m));
+	v.mag = __dadd_rn(v.mag, __shfl_xor_sync(0xffffffffu, v.mag, m));
+	v.pow = __dadd_rn(v.pow, __shfl_xor_sync(0xffffffffu, v.pow, m));
+}
+
+/* grid (row chunk, stream, chain tile), FQ_CT warps */
+template <int KIND>
+__global__ void __launch_bounds__(FQ_CT * 32)
+k_freq_in(const uint8_t *__restrict__ in, size_t stride, int K, int nrows, const int *__restrict__ rows, int nch,
+          const float2 *__restrict__ nco, FreqPart *__restrict__ part, size_t part_stride)
+{
+	using X = typename FreqX<KIND>::T;
+	constexpr int SB = KIND == IN_U8IQ ? 2 : 4;
+	const int s = blockIdx.y, j = blockIdx.x, nr = rows ? rows[s] : nrows, r0 = j * FREQ_ROWS;
+	if (r0 >= nr) return;
+	const int h = K / 2, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c0 = blockIdx.z * FQ_CT, c = c0 + warp;
+	__shared__ X s_x[2][FQ_KT][FREQ_ROWS + 1];          /* + 1: the staging stores (kk fastest) fall in different banks */
+	__shared__ float2 s_w[2][FQ_KT][FQ_CT];
+	const uint8_t *base = in + (size_t)s * stride;
+	float2 a[FQ_RPL], b[FQ_RPL];
+#pragma unroll
+	for (int i = 0; i < FQ_RPL; i++) a[i] = b[i] = make_float2(0.0f, 0.0f);
+	for (int n0 = 0; n0 < h; n0 += FQ_KT) {
+		__syncthreads();
+		for (int e = threadIdx.x; e < 2 * FQ_KT * FREQ_ROWS; e += FQ_CT * 32) {
+			const int kk = e % FQ_KT, hr = e / FQ_KT, half = hr & 1, r = hr >> 1;
+			X v{};
+			if (n0 + kk < h && r0 + r < nr) v = freq_load<KIND>(base + (size_t)(r0 + r) * K * SB, half * h + n0 + kk);
+			s_x[half][kk][r] = v;
+		}
+		if (threadIdx.x < 2 * FQ_KT * FQ_CT) {
+			const int kk = threadIdx.x % FQ_KT, half = (threadIdx.x / FQ_KT) & 1, cc = threadIdx.x / (2 * FQ_KT);
+			float2 w = make_float2(0.0f, 0.0f);
+			if (n0 + kk < h && c0 + cc < nch) w = nco[((size_t)s * nch + c0 + cc) * K + half * h + n0 + kk];
+			s_w[half][kk][cc] = w;
+		}
+		__syncthreads();
+#pragma unroll 4
+		for (int kk = 0; kk < FQ_KT; kk++) {
+			const float2 wa = s_w[0][kk][warp], wb = s_w[1][kk][warp];
+#pragma unroll
+			for (int i = 0; i < FQ_RPL; i++) {
+				freq_mac(a[i], s_x[0][kk][lane + 32 * i], wa);
+				freq_mac(b[i], s_x[1][kk][lane + 32 * i], wb);
+			}
+		}
+	}
+	FreqPart v{ 0.0, 0.0, 0.0, 0.0 };
+#pragma unroll
+	for (int i = 0; i < FQ_RPL; i++) {
+		if (r0 + lane + 32 * i >= nr) continue;
+		const double ar = a[i].x, ai = a[i].y, br = b[i].x, bi = b[i].y;
+		const double pa = __dadd_rn(__dmul_rn(ar, ar), __dmul_rn(ai, ai)), pb = __dadd_rn(__dmul_rn(br, br), __dmul_rn(bi, bi));
+		v.re = __dadd_rn(v.re, __dadd_rn(__dmul_rn(br, ar), __dmul_rn(bi, ai)));
+		v.im = __dadd_rn(v.im, __dsub_rn(__dmul_rn(bi, ar), __dmul_rn(br, ai)));
+		v.mag = __dadd_rn(v.mag, __dmul_rn(__dsqrt_rn(pa), __dsqrt_rn(pb)));
+		v.pow = __dadd_rn(v.pow, __dadd_rn(pa, pb));
+	}
+	for (int m = 16; m; m >>= 1) freq_shfl_add(v, m);
+	if (lane == 0 && c < nch) part[((size_t)s * part_stride + j) * nch + c] = v;
+}
+
+/* one thread per chain: its chunks in order; chains not measured (on[g] == 0) report nothing */
+__global__ void __launch_bounds__(256)
+k_freq_fin(int nrows, const int *__restrict__ rows, int nch, int nstreams, const int *__restrict__ on, const FreqPart *__restrict__ part,
+           size_t part_stride, FreqChan *__restrict__ out)
+{
+	const size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+	if (g >= (size_t)nstreams * nch) return;
+	const int s = (int)(g / nch), c = (int)(g % nch), n = rows ? rows[s] : nrows;
+	FreqChan r{ 0, 0.0, 0.0, 0.0, 0.0 };
+	if (on[g]) {
+		r.pairs = (unsigned long long)n;
+		for (int j = 0; j < (n + FREQ_ROWS - 1) / FREQ_ROWS; j++) {
+			const FreqPart p = part[((size_t)s * part_stride + j) * nch + c];
+			r.s_re = __dadd_rn(r.s_re, p.re);
+			r.s_im = __dadd_rn(r.s_im, p.im);
+			r.mag_sum = __dadd_rn(r.mag_sum, p.mag);
+			r.power_sum = __dadd_rn(r.power_sum, p.pow);
+		}
+	}
+	out[g] = r;
+}
+
+template <int KIND>
+static int launch_freq_input_t(const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nch, int nstreams, const float2 *nco,
+                               const int *on, FreqPart *part, size_t part_stride, FreqChan *out, cudaStream_t stream, int &launched)
+{
+	const unsigned nchunk = (unsigned)((nrows + FREQ_ROWS - 1) / FREQ_ROWS);
+	if (nchunk == 0 || nchunk > part_stride) return (int)cudaErrorInvalidValue;
+	k_freq_in<KIND><<<dim3(nchunk, nstreams, (nch + FQ_CT - 1) / FQ_CT), FQ_CT * 32, 0, stream>>>(in, stride, K, nrows, rows, nch, nco, part,
+	                                                                                              part_stride);
+	const size_t nchain = (size_t)nstreams * nch;
+	k_freq_fin<<<(unsigned)((nchain + 255) / 256), 256, 0, stream>>>(nrows, rows, nch, nstreams, on, part, part_stride, out);
+	launched += 2;
+	return (int)cudaGetLastError();
+}
+
+int launch_freq_input(int in_kind, const uint8_t *in, size_t stride, int K, int nrows, const int *rows, int nch, int nstreams, const float *nco,
+                      const int *on, FreqPart *part, size_t part_stride, FreqChan *out, cudaStream_t stream, int &launched)
+{
+	const float2 *nco2 = reinterpret_cast<const float2 *>(nco);
+	if (in_kind == IN_KIND_U8IQ)
+		return launch_freq_input_t<IN_U8IQ>(in, stride, K, nrows, rows, nch, nstreams, nco2, on, part, part_stride, out, stream, launched);
+	if (in_kind == IN_KIND_CS16IQ)
+		return launch_freq_input_t<IN_CS16IQ>(in, stride, K, nrows, rows, nch, nstreams, nco2, on, part, part_stride, out, stream, launched);
+	return launch_freq_input_t<IN_F32REAL>(in, stride, K, nrows, rows, nch, nstreams, nco2, on, part, part_stride, out, stream, launched);
+}
+
 /* Moving streams (acb_save_streams / acb_load_streams): stream list[i]'s device regions to and from record i of a staging
  * buffer.  blockIdx.y is the record; blockIdx.x walks the regions in SP_CHUNK pieces (R.chunk0[k] is region k's first).
  * A piece whose two addresses and ends are all 16-byte aligned moves in 16-byte vectors, any other in 4-byte words (the

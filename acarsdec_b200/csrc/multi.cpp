@@ -450,6 +450,22 @@ extern "C" int acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, 
 	return ACB_OK;
 }
 
+/* each part's table, placed at the global indices of its chains */
+extern "C" int acb_multi_get_freq_stats(acb_multi_t *m, acb_chan_freq_t *out, size_t n, int reset)
+{
+	if (!m || !out) return fail(ACB_ERR_ARG, "null argument");
+	const int nch = m->cfg.nch;
+	if (n < (size_t)m->cfg.nstreams * nch) return fail(ACB_ERR_ARG, "n=%zu < nstreams*nch", n);
+	std::vector<acb_chan_freq_t> part;
+	for (auto &p : m->parts) {
+		part.resize((size_t)p.ns * p.nc);
+		if (int r = acb_get_freq_stats(p.ctx, part.data(), part.size(), reset)) return r;
+		for (int s = 0; s < p.ns; s++)
+			for (int c = 0; c < p.nc; c++) out[(size_t)(p.s0 + s) * nch + p.c0 + c] = part[(size_t)s * p.nc + c];
+	}
+	return ACB_OK;
+}
+
 /* ---- moving streams: a blob is the one a single context of cfg gives, whatever the split ----
  * A stream split saves each stream on the part that owns it (every part has cfg's fingerprint but nstreams).  In a
  * channel split every part holds every stream but only channels [c0, c0 + nc) of it, in tables laid out for nc channels;
@@ -558,6 +574,8 @@ static void chan_record(const MvHead &h, const MvLayout &F, const MvLayout &P, i
 		if (!to_full || first) mv(part + P.off_lin, full + F.off_lin, sizeof(acb_input_level_t));
 		mv(part + P.off_lch, full + F.off_lch + (size_t)c0 * sizeof(acb_chan_level_t), (size_t)nc * sizeof(acb_chan_level_t));
 	}
+	if (h.flags & ACB_FLAG_FREQ_STATS)
+		mv(part + P.off_fch, full + F.off_fch + (size_t)c0 * sizeof(acb_chan_freq_t), (size_t)nc * sizeof(acb_chan_freq_t));
 }
 
 /* the bins of a full record's wideband plan (0 for a stream not on the raster, whose plan is unused) */

@@ -159,6 +159,12 @@ typedef struct {
                                          each submit already holds.  Any input kind and channelizer form, with or without
                                          ACB_FLAG_DECODE_STATS; messages, envelope, chain states and decode statistics are
                                          unchanged.  Without it acb_get_level_stats returns ACB_ERR_ARG. */
+#define ACB_FLAG_FREQ_STATS 1024      /* measure each chain's carrier offset from its planned frequency (acb_chan_freq_t,
+                                         acb_get_freq_stats, acb_freq_error): how far off frequency each receiver is tuned,
+                                         from the phase rotation of the channel's carrier within each row.  Any input kind
+                                         and channelizer form, with or without the other statistics flags; messages,
+                                         envelope, chain states, decode and level statistics are unchanged.  Without it
+                                         acb_get_freq_stats returns ACB_ERR_ARG. */
 
 /* One decoded block, after parity/CRC repair: msgblk_t (acarsdec.h:48-57) without the queue
  * link, plus where it came from.  `txt` is parity-stripped (acars.c:200). */
@@ -467,7 +473,8 @@ int acb_set_state(acb_ctx_t *ctx, int stream, int chn, const acb_chan_state_t *i
  *   - its nch chain states (the frame being assembled, the PLL, the bit clock);
  *   - the channelizer's input side: the u8 taps > K history, or the streaming kinds' history and carried remainder;
  *   - its channel tables and fast plan, copied as the context holds them (no replanning);
- *   - with ACB_FLAG_DECODE_STATS its decode counts, with ACB_FLAG_LEVEL_STATS its level tables and open 1024-row windows.
+ *   - with ACB_FLAG_DECODE_STATS its decode counts, with ACB_FLAG_LEVEL_STATS its level tables and open 1024-row windows,
+ *     with ACB_FLAG_FREQ_STATS its chains' frequency sums, planned frequencies and NCO steps.
  * Records have one size per configuration.  The exact tables dominate it: nch * taps_pad * 8 bytes (taps_pad: taps
  * rounded up to 16 bytes of input), e.g. about 52 MB per stream at K = 1600, 256 channels, taps = 16K.
  * The format is little-endian and opaque; it carries a magic, a format version, the fingerprint below and a CRC-32, and
@@ -495,7 +502,7 @@ int acb_save_streams(acb_ctx_t *ctx, const int *streams, int n, void *blob, size
  * and, when a save or load needs more staging than the context has used so far, for the allocation (which synchronises
  * the device: save or load the largest set once up front to avoid it in a live pipeline).
  * Refused with ACB_ERR_ARG, the context unchanged, unless the format version and the CRC match, and the input kind, K,
- * taps, nch, channelizer form, the ACB_FLAG_DECODE_STATS and ACB_FLAG_LEVEL_STATS bits and (streaming kinds) the
+ * taps, nch, channelizer form, the ACB_FLAG_DECODE_STATS, ACB_FLAG_LEVEL_STATS and ACB_FLAG_FREQ_STATS bits and (streaming kinds) the
  * emission-group unit and period match the context's.  nstreams, max_blocks and the device may differ. */
 int acb_load_streams(acb_ctx_t *ctx, const int *streams, int n, const void *blob, size_t size);
 /* A blob's fingerprint; host only (no device, no context).  ACB_ERR_ARG for a wrong magic or version, a size that does
@@ -504,7 +511,7 @@ typedef struct {
 	int in_kind;              /* 0 u8 IQ, 1 real, 2 CS16 */
 	int K, taps, nch;         /* taps as the context runs it (K for taps = 0) */
 	int form;                 /* the channelizer form: 0 EXACT, 1 GENERIC, 2 DFT, 3 RDFT, 4 OVL_FAST, 5 OVL_RDFT, 6 WB, 7 WB_REAL */
-	int flags;                /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS bits of the context */
+	int flags;                /* ACB_FLAG_DECODE_STATS | ACB_FLAG_LEVEL_STATS | ACB_FLAG_FREQ_STATS bits of the context */
 	int group_unit;           /* streaming kinds: ACB_GROUP_*; u8: 0 */
 	uint64_t group_period;
 	int count;                /* records */
@@ -603,6 +610,45 @@ typedef struct {
  * window, queued behind the work in flight, and no other stream's.  ACB_ERR_ARG without ACB_FLAG_LEVEL_STATS. */
 int acb_get_level_stats(acb_ctx_t *ctx, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset);
 
+/* Frequency error (ACB_FLAG_FREQ_STATS): how far each channel's AM carrier sits from the frequency the planner placed it
+ * at, and so how far off frequency the receiver is tuned.
+ *
+ * Per chain (s, c), over the same rows the level tables count (every output row m a covered submit produced for stream
+ * s, with its own K input samples [m*K, (m+1)*K), converted as acb_input_level_t documents; the taps > K history is not
+ * used).  With h = K/2 (rounded down: an odd K leaves the row's last sample out) and w the chain's NCO table,
+ *   a_m = sum_{n<h} x[mK+n] w[n],   b_m = sum_{n<h} x[mK+h+n] w[h+n],   w[n] = (float)cos(step n) - j (float)sin(step n),
+ * a_m and b_m in float, the row's terms and the sums in double:
+ *   pairs += 1,  s_re + j s_im += b_m conj(a_m),  mag_sum += |a_m| |b_m|,  power_sum += |a_m|^2 + |b_m|^2.
+ * step is the offset, in radians per input sample, of the channel from the tuner centre that the chain's mixer removes:
+ * 2 pi ((float)Fr - (float)Fc) / rate for the IQ planners (acb_set_plan*, acb_set_plan_cs16), and for real input the
+ * mirror image of air.c's IF, -2 pi (Fc - Fr + rate/4) / rate, since the real front-end's IF is spectrally inverted.
+ * Either way a carrier above freq_hz turns s positive (counter-clockwise) for every input kind.  freq_hz is the RF
+ * frequency the mixer centres: Fc plus the IQ offset, or Fr for real input.  The planners record both for every chain;
+ * a stream whose table came from acb_set_wf has freq_hz = step = 0 and is not measured (pairs stays 0).  A re-plan
+ * takes effect for the rows after it.
+ *
+ * The offset of a chain is rate * atan2(s_im, s_re) / (2 pi h) Hz, with rate = K * 12500: unambiguous within
+ * +-rate / (2h), +-12.5 kHz at even K; a carrier further out aliases by multiples of rate / h.  |s| / mag_sum is in
+ * [0, 1]: near 1 for a chain with a carrier, near 0 for one with noise only.  The tables cover exactly the submits
+ * acb_collect / acb_sync have covered; envelope input (acb_submit_dm_host) adds nothing. */
+typedef struct {
+	uint64_t pairs;        /* rows measured */
+	double   s_re, s_im;   /* sum of b_m conj(a_m) */
+	double   mag_sum;      /* sum of |a_m| |b_m| */
+	double   power_sum;    /* sum of |a_m|^2 + |b_m|^2 */
+	double   freq_hz;      /* the chain's planned RF frequency (0: not measured) */
+	double   step;         /* the NCO's step, radians per input sample */
+} acb_chan_freq_t;
+/* Fills out[s*nch + c] for every chain; n >= nstreams*nch.  reset != 0 clears the sums after reading (freq_hz and step
+ * describe the plan and stay); acb_reset clears every chain's sums, acb_reset_stream that stream's, queued behind the
+ * work in flight.  ACB_ERR_ARG without ACB_FLAG_FREQ_STATS. */
+int acb_get_freq_stats(acb_ctx_t *ctx, acb_chan_freq_t *out, size_t n, int reset);
+/* The offsets, coherences and frequency error of one stream's nch chains (host only): offset_hz[c] and coherence[c] as
+ * above (0 for a chain with pairs == 0), and *ppm = 1e6 * sum_c |s_c| offset_c / freq_hz_c / sum_c |s_c| over the chains
+ * with pairs > 0 (0 when there is none).  Any output may be NULL.  K is the context's (the offset's scale is
+ * K * 12500 / (2 pi floor(K/2))).  ACB_ERR_ARG for a NULL table, nch < 1 or K < 2. */
+int acb_freq_error(const acb_chan_freq_t *ch, int nch, int K, double *offset_hz, double *coherence, double *ppm);
+
 /* ---- one process, several GPUs (the C host's way to a whole node; SURVEY.md §8e) ----
  *
  * acb_multi_* fronts one context per device.  Two ways to cut the work, neither with any device-to-device
@@ -666,6 +712,8 @@ int  acb_multi_get_decode_stats(acb_multi_t *m, acb_decode_stats_t *out, size_t 
 /* acb_get_level_stats over the parts, indexed globally.  A stream split takes each part's streams.  In a channel split
  * every part reads the same samples, so in[] comes from part 0; ch[] from each part's channels. */
 int  acb_multi_get_level_stats(acb_multi_t *m, acb_input_level_t *in, size_t n_in, acb_chan_level_t *ch, size_t n_ch, int reset);
+/* acb_get_freq_stats over the parts, indexed by global stream and channel: out[s*nch + c], n >= nstreams*nch */
+int  acb_multi_get_freq_stats(acb_multi_t *m, acb_chan_freq_t *out, size_t n, int reset);
 /* acb_save_streams / acb_load_streams over the parts.  A blob is the one a single context of cfg would give, whatever the
  * split, so streams move freely between single contexts, stream splits and channel splits.  A stream split takes each
  * stream's record from (gives it to) the part that owns it.  A channel split assembles each stream's nch chains, tables
